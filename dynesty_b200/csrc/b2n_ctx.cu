@@ -10,11 +10,15 @@ static std::mutex g_smem_mu;
 static std::map<std::pair<int, const void*>, size_t> g_smem_limit;
 
 int b2n_func_smem(b2n_ctx* ctx, const void* func, size_t bytes) {
-    if (bytes <= 48 * 1024) return B2N_OK;                      // the default limit needs no opt-in
     std::lock_guard<std::mutex> lk(g_smem_mu);
     size_t& cur = g_smem_limit[std::make_pair(ctx->device, func)];
     if (bytes <= cur) return B2N_OK;
-    B2N_CUDA(ctx, cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    // the default 48 KB limit covers the kernel's static shared memory AND the dynamic bytes: a launch just under
+    // 48 KB of dynamic memory still needs the opt-in when the kernel has __shared__ variables of its own
+    cudaFuncAttributes fa;
+    B2N_CUDA(ctx, cudaFuncGetAttributes(&fa, func));
+    if (bytes + fa.sharedSizeBytes > 48 * 1024)
+        B2N_CUDA(ctx, cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     cur = bytes;
     return B2N_OK;
 }

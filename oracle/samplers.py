@@ -226,7 +226,7 @@ def unif_chain(loglstar, multi, model, stream, ndim, nonbounded=None,
     K = multi.nells
     probs = np.exp(multi.logvol_ells - multi.logvol)
     cum = np.cumsum(probs)
-    ncall = 0
+    ncall = nprop = 0
     nb = None if nonbounded is None else nonbounded[:nc]
     for _ in range(max_tries):
         if K == 1:                                                # bounding.py:543-550
@@ -243,6 +243,7 @@ def unif_chain(loglstar, multi, model, stream, ndim, nonbounded=None,
                         raise RuntimeError('Ellipsoid check failed q=0')
                 if q == 1 or stream.uniform() < 1. / q:
                     break
+        nprop += 1                                                # points the bound proposed
         if not unitcheck(x, nb):                                  # :314
             continue
         u = x if nc == ndim else np.concatenate((x, stream.uniforms(ndim - nc)))
@@ -250,5 +251,5 @@ def unif_chain(loglstar, multi, model, stream, ndim, nonbounded=None,
         logl = float(model.loglike(v))
         ncall += 1
         if logl > loglstar:
-            return dict(u=u, v=v, logl=logl, ncall=ncall, ticks=stream.tick)
+            return dict(u=u, v=v, logl=logl, ncall=ncall, nprop=nprop, ticks=stream.tick)
     raise RuntimeError("unif_chain: no point found")
