@@ -116,6 +116,10 @@ __device__ __forceinline__ double loglike_sm(const B2nModel& m, const ModelSm& m
         return pow(2.0 + warp_prod(pr), m.s1);
     } else if (LIKE == B2N_LIKE_REGION2D) {
         return region2d_logl(m.s0, b2n_sm[ov], b2n_sm[ov + 1]);
+#ifdef B2N_USER_MODEL
+    } else if (LIKE == B2N_LIKE_USER) {
+        return b2n_user_loglike(&b2n_sm[ov], &b2n_sm[od], n, m.lv0, lane);
+#endif
     } else {  // SHELLS
         double a = 0.0, b = 0.0;
         for (int i = lane; i < n; i += 32) {
@@ -270,6 +274,7 @@ __device__ __forceinline__ void stage_matrix(const double* __restrict__ g, int o
     }
 }
 
+#ifndef __CUDACC_RTC__
 // shared by the chain entry points (defined in b2n_rwalk.cu)
 int b2n_build_worklist(b2n_ctx* ctx, int64_t Q, const int32_t* ell, int K, int chains_per_cta,
                        std::vector<int>& order, std::vector<int3>& cta);
@@ -277,3 +282,4 @@ void b2n_chain_grid(const b2n_ctx* ctx, int64_t Q, int max_warps, int& chains_pe
 // worklist on the device: cached for the single-ellipsoid case, else built on the host and uploaded
 int b2n_worklist_dev(b2n_ctx* ctx, int64_t Q, const int32_t* ell, int K, int chains_per_cta, const void** dorder,
                      const void** dcta, unsigned* ncta);
+#endif

@@ -1,12 +1,22 @@
 // b2n_common.cuh -- context, scratch memory and small device helpers shared by
 // all translation units of libb200nest.so (sm_90a only).
+//
+// Everything host-side (the context, scratch buffers, staging helpers) is hidden from NVRTC (__CUDACC_RTC__): the
+// device-only part -- B2nModel, PeerSet, B2nDyn and the warp helpers -- is also compiled at run time into the
+// kernels of a user likelihood (b2n_user_kernels.cuh).
 #pragma once
+#ifndef __CUDACC_RTC__
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
+#else
+#ifndef INFINITY
+#define INFINITY __int_as_float(0x7f800000)
+#endif
+#endif
 #include "../../include/b200nest.h"
 
 #define B2N_WARP 32
@@ -23,6 +33,7 @@ struct B2nModel {
     double s0, s1, s2;
 };
 
+#ifndef __CUDACC_RTC__
 // growable device buffer
 struct DevBuf {
     void* p = nullptr;
@@ -39,6 +50,7 @@ struct DevBuf {
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() { return reinterpret_cast<T*>(p); }
 };
+#endif
 
 // ---- peer exchange (multi-GPU gather fused into the chain kernels, b2n_peer.cu) ----------
 // Window layout: 256-byte header { u64 arrive @0 | u32 err @8 | u32 done @64 } then two slots
@@ -50,6 +62,7 @@ struct PeerSet {               // passed by value to the chain kernels; world ==
     char* base[B2N_MAX_PEERS] = {nullptr};
     unsigned long long target = 0;     // own arrive counter once every rank has arrived
 };
+#ifndef __CUDACC_RTC__
 struct PeerState {
     int world = 0, rank = 0;
     char* win = nullptr;               // own window
@@ -61,6 +74,7 @@ struct PeerState {
     uint64_t off[7] = {0};             // byte offsets of the arrays of the last call
     unsigned int* err_host = nullptr;  // pinned mailbox for the window's err word
 };
+#endif
 
 // ---- device-paced launches (b2n_ns.cu): the per-round arguments of a chain kernel live in HBM,
 // written by the previous kernel on the stream, so that consecutive nested-sampling rounds need
@@ -71,6 +85,7 @@ struct B2nDyn {
     unsigned long long chain0;
     int skip, ncta, doubling, pad;
 };
+#ifndef __CUDACC_RTC__
 struct DynLaunch {
     bool active = false;         // the next chain entry call is device-paced
     bool plan_only = false;      // ... and only reports chains_per_cta (no launch)
@@ -127,7 +142,24 @@ struct b2n_ctx {
     DevBuf wl_order, wl_cta;
     int64_t wl_Q = -1;
     int wl_cpc = 0, wl_ncta = 0;
+    // user likelihoods (b2n_model_create_user): user_fn[model id] = the run-time loaded kernel of every slot of
+    // B2nUserSlot (empty for a registry model); the libraries are unloaded by b2n_free
+    std::vector<std::vector<const void*>> user_fn;
+    std::vector<cudaLibrary_t> user_libs;
 };
+
+// The kernel instantiations a user likelihood is compiled into, in the order of b2n_user_kernel_exprs (b2n_ctx.cu).
+enum B2nUserSlot {
+    B2N_US_EVAL = 0,          // model_eval_kernel
+    B2N_US_UNITCUBE = 1,      // unitcube_kernel
+    B2N_US_UNIF = 2,          // unif_kernel
+    B2N_US_RWALK = 3,         // rwalk_kernel<AX_SMEM = 0>, + 1: AX_SMEM = 1
+    B2N_US_SLICE = 5,         // slice_kernel, + 2 * RANDOM_DIR + AX_SMEM
+    B2N_US_FRIENDS = 9,       // friends_unif_kernel
+    B2N_US_COUNT = 10
+};
+// Launch slot `slot` of the user model `model_id` on the ctx stream (shared-memory opt-in through b2n_func_smem).
+int b2n_user_launch(b2n_ctx* ctx, int model_id, int slot, dim3 grid, dim3 block, size_t smem, void** args);
 // cudaFuncAttributeMaxDynamicSharedMemorySize, raised ONCE per (device, kernel) and never lowered: the attribute is
 // process-wide per device, so two contexts of different problem sizes must not shrink each other's limit, and a driver
 // call per launch is a lock every replica thread would queue on (b2n_ctx.cu)
@@ -242,6 +274,7 @@ static inline int b2n_finish(b2n_ctx* ctx) {
     if (ctx->ptr_mode == B2N_PTR_HOST) B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2N_OK;
 }
+#endif  // !__CUDACC_RTC__
 
 // ---- warp helpers ----------------------------------------------------------------
 __device__ __forceinline__ double warp_sum(double v) {

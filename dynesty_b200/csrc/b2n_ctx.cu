@@ -1,6 +1,6 @@
 // b2n_ctx.cu -- context lifetime, model registry, resident bound, batched model
 // evaluation.  Part of libb200nest.so (C ABI in include/b200nest.h).
-#include "b2n_device.cuh"
+#include "b2n_eval_kernel.cuh"
 #include <algorithm>
 #include <time.h>
 #include <map>
@@ -20,6 +20,22 @@ int b2n_func_smem(b2n_ctx* ctx, const void* func, size_t bytes) {
     if (bytes + fa.sharedSizeBytes > 48 * 1024)
         B2N_CUDA(ctx, cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     cur = bytes;
+    return B2N_OK;
+}
+
+// A run-time loaded kernel is gone once its library is unloaded, and a later library may reuse its handle: drop
+// the remembered limit so that a new kernel at the same address gets its own opt-in.
+static void b2n_func_smem_forget(int device, const void* func) {
+    std::lock_guard<std::mutex> lk(g_smem_mu);
+    g_smem_limit.erase(std::make_pair(device, func));
+}
+
+int b2n_user_launch(b2n_ctx* ctx, int model_id, int slot, dim3 grid, dim3 block, size_t smem, void** args) {
+    if (model_id < 0 || model_id >= (int)ctx->user_fn.size() || (int)ctx->user_fn[model_id].size() != B2N_US_COUNT)
+        return b2n_fail(ctx, B2N_ERR_ARG, "not a user model (b2n_model_create_user)");
+    const void* f = ctx->user_fn[model_id][slot];
+    B2N_TRY(b2n_func_smem(ctx, f, smem));
+    B2N_CUDA(ctx, cudaLaunchKernel(f, grid, block, args, smem, ctx->stream));
     return B2N_OK;
 }
 
@@ -104,6 +120,9 @@ void b2n_free(b2n_ctx* ctx) {
     b2n_ns_release(ctx);
     b2n_friends_release(ctx);
     for (void* p : ctx->model_allocs) cudaFree(p);
+    for (const auto& fns : ctx->user_fn)
+        for (const void* f : fns) b2n_func_smem_forget(ctx->device, f);
+    for (cudaLibrary_t l : ctx->user_libs) cudaLibraryUnload(l);
     if (ctx->ev0) { cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1); }
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -234,6 +253,72 @@ int b2n_model_create(b2n_ctx* ctx, const b2n_model_desc* d, int32_t* id) {
     B2N_TRY(upload(ctx, d->like_vec1, n, &m.lv1));
     B2N_TRY(upload(ctx, d->like_mat, n * n, &m.lmat));
     ctx->models.push_back(m);
+    ctx->user_fn.emplace_back();
+    *id = (int32_t)ctx->models.size() - 1;
+    return B2N_OK;
+}
+
+// NVRTC name expressions of the user-likelihood kernels, indexed by B2nUserSlot (B2N_LIKE_USER = 5)
+static const char* const g_user_exprs[B2N_US_COUNT] = {
+    "model_eval_kernel<5>",
+    "unitcube_kernel<5>",
+    "unif_kernel<5>",
+    "rwalk_kernel<5, false, false>",
+    "rwalk_kernel<5, true, false>",
+    "slice_kernel<5, false, false, false>",
+    "slice_kernel<5, false, true, false>",
+    "slice_kernel<5, true, false, false>",
+    "slice_kernel<5, true, true, false>",
+    "friends_unif_kernel<5>",
+};
+
+int b2n_user_kernel_exprs(const char* const** exprs, int32_t* count) {
+    if (!exprs || !count) return B2N_ERR_ARG;
+    *exprs = g_user_exprs;
+    *count = B2N_US_COUNT;
+    return B2N_OK;
+}
+
+int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double* params, int64_t nparams,
+                          const void* image, size_t image_bytes, const char* const* lowered_names, int32_t* id) {
+    if (!ctx || !d || !id || d->ndim < 1 || d->like_kind != B2N_LIKE_USER || nparams < 0 || (nparams > 0 && !params) ||
+        !image || image_bytes == 0 || !lowered_names)
+        return B2N_ERR_ARG;
+    if (d->prior_kind < 0 || d->prior_kind > B2N_PRIOR_NORMAL_PPF) return B2N_ERR_ARG;
+    if (d->prior_kind != B2N_PRIOR_IDENTITY && (!d->prior_p0 || !d->prior_p1)) return B2N_ERR_ARG;
+    for (int s = 0; s < B2N_US_COUNT; s++)
+        if (!lowered_names[s]) return B2N_ERR_ARG;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaLibrary_t lib = nullptr;
+    B2N_CUDA(ctx, cudaLibraryLoadData(&lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0));
+    ctx->user_libs.push_back(lib);
+    std::vector<const void*> fns(B2N_US_COUNT);
+    for (int s = 0; s < B2N_US_COUNT; s++) {
+        cudaKernel_t k = nullptr;
+        const cudaError_t e = cudaLibraryGetKernel(&k, lib, lowered_names[s]);
+        if (e != cudaSuccess) {
+            snprintf(ctx->err, sizeof(ctx->err), "user model: kernel %s (%s) not in the image: %s", g_user_exprs[s],
+                     lowered_names[s], cudaGetErrorString(e));
+            return B2N_ERR_ARG;
+        }
+        fns[s] = (const void*)k;
+    }
+    const size_t n = d->ndim;
+    B2nModel m;
+    memset(&m, 0, sizeof(m));
+    m.ndim = d->ndim;
+    m.prior_kind = d->prior_kind;
+    m.like_kind = B2N_LIKE_USER;
+    B2N_TRY(upload(ctx, d->prior_p0, n, &m.pp0));
+    B2N_TRY(upload(ctx, d->prior_p1, n, &m.pp1));
+    if (nparams > 0) {
+        // the chain kernels stage lv0[0, ndim) into shared memory for every model: pad to ndim with zeros
+        std::vector<double> pv(std::max<size_t>((size_t)nparams, n), 0.0);
+        std::copy(params, params + nparams, pv.begin());
+        B2N_TRY(upload(ctx, pv.data(), pv.size(), &m.lv0));
+    }
+    ctx->models.push_back(m);
+    ctx->user_fn.push_back(fns);
     *id = (int32_t)ctx->models.size() - 1;
     return B2N_OK;
 }
@@ -308,29 +393,6 @@ extern "C" {
 
 }  // extern "C"
 
-// ---- batched model evaluation: one warp per point -------------------------------------
-template <int LIKE>
-__global__ void __launch_bounds__(256) model_eval_kernel(B2nModel m, const double* __restrict__ u,
-                                                         int64_t M, double* __restrict__ v,
-                                                         double* __restrict__ logl) {
-    extern __shared__ double sm[];
-    const int n = m.ndim;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int wpb = blockDim.x >> 5;
-    double* vv = sm + (size_t)warp * 2 * n;
-    double* work = vv + n;
-    for (int64_t p = (int64_t)blockIdx.x * wpb + warp; p < M; p += (int64_t)gridDim.x * wpb) {
-        for (int i = lane; i < n; i += 32) {
-            const double x = prior_1d(m, i, u[p * n + i]);
-            vv[i] = x;
-            if (v) v[p * n + i] = x;
-        }
-        __syncwarp();
-        const double l = warp_loglike<LIKE>(m, m.lmat, vv, work, lane);
-        if (lane == 0) logl[p] = l;
-        __syncwarp();
-    }
-}
 
 extern "C" int b2n_model_eval(b2n_ctx* ctx, int32_t id, const double* u, int64_t M, double* v,
                               double* logl) {
@@ -348,12 +410,18 @@ extern "C" int b2n_model_eval(b2n_ctx* ctx, int32_t id, const double* u, int64_t
     const size_t smem = (size_t)wpb * 2 * n * sizeof(double);
     int64_t blocks = (M + wpb - 1) / wpb;
     if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    if (m.like_kind == B2N_LIKE_USER) {
+        int64_t M_ = M;
+        void* args[] = {(void*)&m, (void*)&du, (void*)&M_, (void*)&dv, (void*)&dl};
+        B2N_TRY(b2n_user_launch(ctx, id, B2N_US_EVAL, dim3((unsigned)blocks), dim3(threads), smem, args));
+    } else {
 #define CALL(L)                                                                                   \
     if (smem > 48 * 1024)                                                                          \
         B2N_TRY(b2n_func_smem(ctx, (const void*)(model_eval_kernel<L>), (size_t)(smem))); \
     model_eval_kernel<L><<<(unsigned)blocks, threads, smem, ctx->stream>>>(                         \
         m, (const double*)du, M, (double*)dv, (double*)dl);
-    B2N_DISPATCH_LIKE(m.like_kind, CALL)
+        B2N_DISPATCH_LIKE(m.like_kind, CALL)
+    }
 #undef CALL
     B2N_LAUNCH_CHECK(ctx);
     B2N_TRY(b2n_out_done(ctx, v, dv, M * n * sizeof(double)));

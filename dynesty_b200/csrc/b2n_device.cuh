@@ -97,6 +97,12 @@ __device__ __forceinline__ double region2d_logl(double shape, double x, double y
     return sin(x * mult) * sin(y * mult);
 }
 
+#ifdef B2N_USER_MODEL
+// the user likelihood of a run-time compiled model (contract: include/b200nest.h, b2n_model_create_user),
+// defined after b2n_user_kernels.cuh in the same NVRTC program
+__device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane);
+#endif
+
 // ---- log-likelihood, evaluated cooperatively by one warp ---------------------------
 // v: warp-private shared vector (n).  work: warp-private shared scratch (n).
 // lmat: pointer to the n x n matrix for GAUSS_PREC (shared or global).
@@ -135,6 +141,10 @@ __device__ __forceinline__ double warp_loglike(const B2nModel& m, const double* 
         return pow(2.0 + p, m.s1);
     } else if (LIKE == B2N_LIKE_REGION2D) {
         return region2d_logl(m.s0, v[0], v[1]);
+#ifdef B2N_USER_MODEL
+    } else if (LIKE == B2N_LIKE_USER) {
+        return b2n_user_loglike(v, work, n, m.lv0, lane);
+#endif
     } else {  // SHELLS
         double a = 0.0, b = 0.0;
         for (int i = lane; i < n; i += 32) {
@@ -153,7 +163,8 @@ __device__ __forceinline__ double warp_loglike(const B2nModel& m, const double* 
     }
 }
 
-// kernel dispatch on the likelihood kind
+// kernel dispatch on the likelihood kind (B2N_LIKE_USER never reaches it: its kernels are loaded at run time and
+// launched through b2n_user_launch)
 #define B2N_DISPATCH_LIKE(kind, CALL)                                   \
     switch (kind) {                                                     \
         case B2N_LIKE_GAUSS_PREC: { CALL(B2N_LIKE_GAUSS_PREC); } break; \

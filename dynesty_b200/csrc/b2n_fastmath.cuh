@@ -12,9 +12,11 @@
 // The file compiles for the host as well (B2N_HD), which is how the accuracy test runs without a GPU; on the
 // host the hardware approximations are emulated by rounding an exact result to float precision first.
 #pragma once
+#ifndef __CUDACC_RTC__
 #include <stdint.h>
 #include <string.h>
 #include <math.h>
+#endif
 
 #ifdef __CUDACC__
 #define B2N_HD __host__ __device__ __forceinline__

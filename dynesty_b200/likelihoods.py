@@ -10,6 +10,9 @@ same object can be handed to dynesty's own ``NestedSampler`` as
 ``loglikelihood=model.loglikelihood, prior_transform=model.prior_transform``
 (unit-cube warm-up phase, initial live points) while the B200 samplers pick up
 the descriptor for the in-kernel evaluation.
+
+``DeviceModel.from_cuda`` opens the registry: the log-likelihood is then user CUDA code compiled into the same
+kernels at run time (NVRTC, ``usermodel.py``).
 """
 import ctypes as C
 import math
@@ -48,6 +51,49 @@ class DeviceModel:
         d.like_s0, d.like_s1, d.like_s2 = self.s
         return d
 
+    @classmethod
+    def from_cuda(cls, ndim, source, params=None, prior_kind=_lib.PRIOR_IDENTITY, prior_p0=None, prior_p1=None,
+                  name='user'):
+        """A model whose log-likelihood is user CUDA code, compiled into the proposal kernels at run time.
+
+        ``source`` defines ONE warp-cooperative device function::
+
+            __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane);
+
+        * all 32 lanes of a warp call it (``lane`` = 0..31) and it must return the same value on every lane;
+        * ``v``: the prior-transformed point, ``n`` = ndim doubles in warp-private shared memory (read only);
+        * ``work``: ``n`` doubles of warp-private shared scratch;
+        * ``p``: ``params`` (float64) in device memory, or NULL when ``params`` is None;
+        * ``b2n_warp_sum`` / ``b2n_warp_prod`` / ``b2n_warp_max`` / ``b2n_warp_min`` reduce over the warp.
+
+        A sum over dimensions is split over the lanes and reduced::
+
+            __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane) {
+                double s = 0.0;
+                for (int i = lane; i < n; i += 32) s += (v[i] - p[i]) * (v[i] - p[i]);
+                return -0.5 * b2n_warp_sum(s);
+            }
+
+        A scalar formula is computed by lane 0 and broadcast::
+
+            __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane) {
+                double l = 0.0;
+                if (lane == 0) l = -0.5 * (v[0] * v[0] + 100.0 * (v[1] - v[0] * v[0]) * (v[1] - v[0] * v[0]));
+                return __shfl_sync(0xffffffffu, l, 0);
+            }
+
+        The prior is one of the registry's (``prior_kind`` with per-dimension ``prior_p0`` / ``prior_p1``).  The
+        model is accepted wherever a registry model is: every sampler, the device-resident rounds, the dynamic
+        sampler, replicas; random walks run on the warp-per-chain kernel.  The source is compiled with NVRTC for
+        sm_90a (once per process, ``usermodel.compile_user``); a compile error raises
+        ``usermodel.UserModelCompileError`` carrying NVRTC's log.  Pickling keeps ``source`` and ``params``.
+        """
+        m = cls(ndim, prior_kind, _lib.LIKE_USER, prior_p0=prior_p0, prior_p1=prior_p1, name=name)
+        m.source = str(source)
+        m.params = None if params is None else f64(np.ravel(params))
+        m.logz_truth = None
+        return m
+
     def ids(self, ctx=None):
         ctx = ctx if ctx is not None else _lib.default_context()
         key = ctx.serial           # (not id(ctx): an address can be reused after a Context is freed)
@@ -55,10 +101,22 @@ class DeviceModel:
             out = []
             for pk in (self.prior_kind, _lib.PRIOR_IDENTITY):
                 mid = C.c_int32(-1)
-                ctx.check(ctx.lib.b2n_model_create(ctx.h, C.byref(self._desc(pk)), C.byref(mid)))
+                if self.like_kind == _lib.LIKE_USER:
+                    self._create_user(ctx, pk, mid)
+                else:
+                    ctx.check(ctx.lib.b2n_model_create(ctx.h, C.byref(self._desc(pk)), C.byref(mid)))
                 out.append(mid.value)
             self._ids[key] = tuple(out)
         return self._ids[key]
+
+    def _create_user(self, ctx, prior_kind, mid):
+        from . import usermodel
+        cm = usermodel.compile_user(self.source)
+        names = (C.c_char_p * len(cm.lowered))(*[s.encode() for s in cm.lowered])
+        prm = self.params
+        ctx.check(ctx.lib.b2n_model_create_user(ctx.h, C.byref(self._desc(prior_kind)), ptr(prm),
+                                                0 if prm is None else prm.size, cm.cubin, len(cm.cubin), names,
+                                                C.byref(mid)))
 
     def model_id(self, ctx=None):
         return self.ids(ctx)[0]

@@ -29,7 +29,18 @@
 #ifndef B200NEST_H_
 #define B200NEST_H_
 
+#ifdef __CUDACC_RTC__
+/* NVRTC (the run-time compiled kernels of a user likelihood) has no C library headers */
+#include <cuda/std/cstdint>
+typedef cuda::std::int32_t int32_t;
+typedef cuda::std::int64_t int64_t;
+typedef cuda::std::uint8_t uint8_t;
+typedef cuda::std::uint32_t uint32_t;
+typedef cuda::std::uint64_t uint64_t;
+#else
+#include <stddef.h>
 #include <stdint.h>
+#endif
 
 #ifdef __cplusplus
 extern "C" {
@@ -103,7 +114,8 @@ double b2n_last_kernel_ms(b2n_ctx* ctx);
 /* ---- device models: the "device-side likelihood callback" -----------------
  * The reference evaluates user Python callables prior_transform(u) and
  * loglikelihood(v) once per proposal (internal_samplers.py:957-958, 1116-1117,
- * 328-329).  Inside a kernel that callback is a closed registry:            */
+ * 328-329).  Inside a kernel that callback is a registry of formulas, plus
+ * user CUDA code compiled at run time (B2N_LIKE_USER, b2n_model_create_user): */
 #define B2N_PRIOR_IDENTITY   0  /* v = u                                          */
 #define B2N_PRIOR_UNIFORM    1  /* v = p0[i] + p1[i]*u   (lo, width)               */
 #define B2N_PRIOR_NORMAL_PPF 2  /* v = p0[i] + p1[i]*ndtri(u)  (mu, sigma)         */
@@ -114,6 +126,7 @@ double b2n_last_kernel_ms(b2n_ctx* ctx);
 #define B2N_LIKE_REGION2D    4  /* the hard-edged 2-D regions of the reference's sampler-uniformity harness
                                    (tests/test_sampling.py:8-23) on (v[0], v[1]), other dims free:
                                    s0 = 0: diamond_logl, s0 = 1: checker_logl; -inf outside           */
+#define B2N_LIKE_USER        5  /* user CUDA code compiled at run time: b2n_model_create_user below     */
 
 typedef struct {
     int32_t ndim;
@@ -135,6 +148,35 @@ int b2n_model_create(b2n_ctx* ctx, const b2n_model_desc* desc, int32_t* model_id
  * Replaces the pool.map of the two callables in sampler.py:148-158. v may be NULL. */
 int b2n_model_eval(b2n_ctx* ctx, int32_t model_id, const double* u, int64_t M,
                    double* v, double* logl);
+
+/* ---- user likelihoods: user CUDA code compiled into the proposal kernels at run time ----------
+ * The user writes ONE warp-cooperative device function,
+ *
+ *     __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane);
+ *
+ *   - all 32 lanes of a warp call it, lane = 0..31, and it must return the same value on every lane;
+ *   - v: the prior-transformed point (n doubles, warp-private shared memory, read only);
+ *   - work: n doubles of warp-private shared scratch (contents undefined on entry);
+ *   - p: the model's parameter array in device memory (nparams doubles of b2n_model_create_user; NULL if none);
+ *   - the warp reductions b2n_warp_sum / b2n_warp_prod / b2n_warp_max / b2n_warp_min are available; a scalar
+ *     likelihood is computed on lane 0 and broadcast with __shfl_sync(0xffffffff, x, 0).
+ * The prior is the registry's (B2N_PRIOR_*, per-dimension p0 / p1).  The caller compiles the chain kernels with
+ * that function as the likelihood -- NVRTC, sm_90a, the program being
+ *     #include "b2n_user_kernels.cuh"  followed by the user's source,
+ * with one name expression per slot of b2n_user_kernel_exprs -- and hands the cubin to b2n_model_create_user.
+ * Every entry point that takes a model id then launches the user's instantiation of the same kernel with the same
+ * grid and shared-memory plan.  b2n_rwalk_batch runs a user model on the warp-per-chain kernel at every ndim (the
+ * lock-step tensor-core kernels exist for the registry only; B2N_RWALK_IMPL=mma gives B2N_ERR_UNSUPPORTED).
+ *
+ * b2n_user_kernel_exprs: the NVRTC name expressions to instantiate, in slot order (host only, static strings).
+ * b2n_model_create_user: desc gives ndim and the prior; desc->like_kind must be B2N_LIKE_USER (like_* ignored).
+ *     image: the cubin (host, image_bytes); lowered_names: the mangled name of every slot, as NVRTC reported it
+ *     for the expression of the same index.  Loads the image on the context's device (unloaded by b2n_free) and
+ *     copies params (host, nparams doubles, may be NULL) to the device. */
+int b2n_user_kernel_exprs(const char* const** exprs, int32_t* count);
+int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* desc, const double* params, int64_t nparams,
+                          const void* image, size_t image_bytes, const char* const* lowered_names,
+                          int32_t* model_id);
 
 /* ---- ellipsoid membership: MultiEllipsoid.within/overlap/contains
  *      (bounding.py:502-523), Ellipsoid.distance_many/contains (:286-305) ----
