@@ -14,7 +14,7 @@ LIBPATH = os.path.join(HERE, 'libb200nest.so')
 
 PTR_HOST, PTR_DEVICE = 0, 1
 DIM_PERIODIC, DIM_REFLECTIVE = 1, 2
-PRIOR_IDENTITY, PRIOR_UNIFORM, PRIOR_NORMAL_PPF = 0, 1, 2
+PRIOR_IDENTITY, PRIOR_UNIFORM, PRIOR_NORMAL_PPF, PRIOR_USER = 0, 1, 2, 3
 LIKE_GAUSS_PREC, LIKE_GAUSS_DIAG, LIKE_EGGBOX, LIKE_SHELLS, LIKE_REGION2D, LIKE_USER = 0, 1, 2, 3, 4, 5
 WARN_IDENTITY_FALLBACK, WARN_DOUBLING, WARN_Q0_SLACK, WARN_UNIF_INEFFICIENT = 1, 2, 4, 8
 
@@ -81,6 +81,8 @@ SYMBOLS = {
     'b2n_user_kernel_exprs': (C.c_int, [C.POINTER(C.POINTER(C.c_char_p)), C.POINTER(_I)]),
     'b2n_model_create_user': (C.c_int, [_P, C.POINTER(ModelDesc), _P, _L, _P, C.c_size_t, C.POINTER(C.c_char_p),
                                         C.POINTER(_I)]),
+    'b2n_model_create_user_ex': (C.c_int, [_P, C.POINTER(ModelDesc), _P, _L, _P, _L, _P, C.c_size_t,
+                                           C.POINTER(C.c_char_p), C.POINTER(_I)]),
     'b2n_membership': (C.c_int, [_P, _P, _L, _I, _P, _P, _I, _I, _P, _P, _P]),
     'b2n_bounding_ellipsoid': (C.c_int, [_P, _P, _L, _I, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_multi_decompose': (C.c_int, [_P, _P, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

@@ -279,19 +279,48 @@ int b2n_user_kernel_exprs(const char* const** exprs, int32_t* count) {
     return B2N_OK;
 }
 
-int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double* params, int64_t nparams,
-                          const void* image, size_t image_bytes, const char* const* lowered_names, int32_t* id) {
+}  // extern "C"
+
+// the zero-padded copy of a user parameter array: the chain kernels stage [0, ndim) of lv0 and pp0 into shared
+// memory for every model
+static int upload_padded(b2n_ctx* ctx, const double* h, int64_t count, size_t n, const double** d) {
+    *d = nullptr;
+    if (count <= 0) return B2N_OK;
+    std::vector<double> pv(std::max<size_t>((size_t)count, n), 0.0);
+    std::copy(h, h + count, pv.begin());
+    return upload(ctx, pv.data(), pv.size(), d);
+}
+
+// b2n_model_create_user(_ex); user_prior: desc->prior_kind == B2N_PRIOR_USER was accepted by the caller
+static int model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double* params, int64_t nparams,
+                             bool user_prior, const double* prior_params, int64_t nprior_params, const void* image,
+                             size_t image_bytes, const char* const* lowered_names, int32_t* id) {
     if (!ctx || !d || !id || d->ndim < 1 || d->like_kind != B2N_LIKE_USER || nparams < 0 || (nparams > 0 && !params) ||
         !image || image_bytes == 0 || !lowered_names)
         return B2N_ERR_ARG;
-    if (d->prior_kind < 0 || d->prior_kind > B2N_PRIOR_NORMAL_PPF) return B2N_ERR_ARG;
-    if (d->prior_kind != B2N_PRIOR_IDENTITY && (!d->prior_p0 || !d->prior_p1)) return B2N_ERR_ARG;
+    if (!user_prior) {
+        if (d->prior_kind < 0 || d->prior_kind > B2N_PRIOR_NORMAL_PPF) return B2N_ERR_ARG;
+        if (d->prior_kind != B2N_PRIOR_IDENTITY && (!d->prior_p0 || !d->prior_p1)) return B2N_ERR_ARG;
+    }
     for (int s = 0; s < B2N_US_COUNT; s++)
         if (!lowered_names[s]) return B2N_ERR_ARG;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaLibrary_t lib = nullptr;
     B2N_CUDA(ctx, cudaLibraryLoadData(&lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0));
     ctx->user_libs.push_back(lib);
+    if (user_prior) {
+        // an image compiled without B2N_USER_PRIOR has no prior call in its kernels: refuse it rather than
+        // sample the placeholder v = u
+        void* marker = nullptr;
+        size_t marker_bytes = 0;
+        if (cudaLibraryGetGlobal(&marker, &marker_bytes, lib, "b2n_user_prior_abi") != cudaSuccess) {
+            cudaGetLastError();          // (not sticky: the context stays usable)
+            snprintf(ctx->err, sizeof(ctx->err),
+                     "user model: prior kind B2N_PRIOR_USER, but the image was compiled without a prior "
+                     "(no b2n_user_prior_abi; compile b2n_user_prior with B2N_USER_PRIOR defined)");
+            return B2N_ERR_ARG;
+        }
+    }
     std::vector<const void*> fns(B2N_US_COUNT);
     for (int s = 0; s < B2N_US_COUNT; s++) {
         cudaKernel_t k = nullptr;
@@ -309,18 +338,34 @@ int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double* p
     m.ndim = d->ndim;
     m.prior_kind = d->prior_kind;
     m.like_kind = B2N_LIKE_USER;
-    B2N_TRY(upload(ctx, d->prior_p0, n, &m.pp0));
-    B2N_TRY(upload(ctx, d->prior_p1, n, &m.pp1));
-    if (nparams > 0) {
-        // the chain kernels stage lv0[0, ndim) into shared memory for every model: pad to ndim with zeros
-        std::vector<double> pv(std::max<size_t>((size_t)nparams, n), 0.0);
-        std::copy(params, params + nparams, pv.begin());
-        B2N_TRY(upload(ctx, pv.data(), pv.size(), &m.lv0));
+    if (user_prior) {
+        B2N_TRY(upload_padded(ctx, prior_params, nprior_params, n, &m.pp0));     // pp1 stays NULL
+    } else {
+        B2N_TRY(upload(ctx, d->prior_p0, n, &m.pp0));
+        B2N_TRY(upload(ctx, d->prior_p1, n, &m.pp1));
     }
+    B2N_TRY(upload_padded(ctx, params, nparams, n, &m.lv0));
     ctx->models.push_back(m);
     ctx->user_fn.push_back(fns);
     *id = (int32_t)ctx->models.size() - 1;
     return B2N_OK;
+}
+
+extern "C" {
+
+int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double* params, int64_t nparams,
+                          const void* image, size_t image_bytes, const char* const* lowered_names, int32_t* id) {
+    return model_create_user(ctx, d, params, nparams, false, nullptr, 0, image, image_bytes, lowered_names, id);
+}
+
+int b2n_model_create_user_ex(b2n_ctx* ctx, const b2n_model_desc* d, const double* params, int64_t nparams,
+                             const double* prior_params, int64_t nprior_params, const void* image,
+                             size_t image_bytes, const char* const* lowered_names, int32_t* id) {
+    if (!d || nprior_params < 0 || (nprior_params > 0 && !prior_params)) return B2N_ERR_ARG;
+    const bool user_prior = d->prior_kind == B2N_PRIOR_USER;
+    if (!user_prior && nprior_params != 0) return B2N_ERR_ARG;
+    return model_create_user(ctx, d, params, nparams, user_prior, prior_params, nprior_params, image, image_bytes,
+                             lowered_names, id);
 }
 
 int b2n_bound_set(b2n_ctx* ctx, int32_t K, int32_t nc, const double* ctrs, const double* ams,

@@ -103,6 +103,21 @@ __device__ __forceinline__ double region2d_logl(double shape, double x, double y
 __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane);
 #endif
 
+#ifdef B2N_USER_PRIOR
+// the user prior transform of a run-time compiled model (B2N_PRIOR_USER; contract: include/b200nest.h,
+// b2n_model_create_user_ex), defined after b2n_user_kernels.cuh in the same NVRTC program
+__device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane);
+
+// v = prior_transform(u) as ONE warp-cooperative call (a joint prior reads every component of u).  The per-element
+// prior_1d / prior_sm of the callers write u itself as a placeholder for B2N_PRIOR_USER; this overwrites it.
+__device__ __forceinline__ void user_prior_warp(const B2nModel& m, const double* u, double* v, double* work,
+                                                int lane) {
+    __syncwarp();
+    b2n_user_prior(u, v, work, m.ndim, m.pp0, lane);
+    __syncwarp();
+}
+#endif
+
 // ---- log-likelihood, evaluated cooperatively by one warp ---------------------------
 // v: warp-private shared vector (n).  work: warp-private shared scratch (n).
 // lmat: pointer to the n x n matrix for GAUSS_PREC (shared or global).

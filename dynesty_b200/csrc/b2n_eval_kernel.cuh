@@ -21,6 +21,13 @@ __global__ void __launch_bounds__(256) model_eval_kernel(B2nModel m, const doubl
             if (v) v[p * n + i] = x;
         }
         __syncwarp();
+#ifdef B2N_USER_PRIOR
+        if (m.prior_kind == B2N_PRIOR_USER) {
+            user_prior_warp(m, u + p * n, vv, work, lane);
+            if (v)
+                for (int i = lane; i < n; i += 32) v[p * n + i] = vv[i];
+        }
+#endif
         const double l = warp_loglike<LIKE>(m, m.lmat, vv, work, lane);
         if (lane == 0) logl[p] = l;
         __syncwarp();

@@ -128,6 +128,11 @@ __global__ void __launch_bounds__(512, 1) rwalk_kernel(const RwalkParams p) {
             }
             ok = __all_sync(B2N_FULL, ok);       // also orders the shared-memory writes above
             if (!ok) { nrej++; continue; }
+#ifdef B2N_USER_PRIOR
+            // a user prior maps the whole proposal at once, clustered and non-clustered dims, with the likelihood
+            // scratch as its work (a rejected proposal needs no v: it consumes no random numbers either way)
+            if (pk == B2N_PRIOR_USER) user_prior_warp(p.m, &b2n_sm[ouprop], &b2n_sm[ovprop], &b2n_sm[od], lane);
+#endif
             // (5) likelihood
             double l;
             if (LIKE == B2N_LIKE_GAUSS_PREC) {
@@ -151,6 +156,9 @@ __global__ void __launch_bounds__(512, 1) rwalk_kernel(const RwalkParams p) {
                 b2n_sm[od + i] = vi - b2n_sm[omu + i];
             }
             __syncwarp();
+#ifdef B2N_USER_PRIOR
+            if (pk == B2N_PRIOR_USER) user_prior_warp(p.m, &b2n_sm[oucur], &b2n_sm[ovcur], &b2n_sm[od], lane);
+#endif
             if (LIKE == B2N_LIKE_GAUSS_PREC) {
                 lcur = fma(-0.5, quadform_full<PREC_SMEM>(Pg, offP, ldP, n, od, lane), p.m.s0);
             } else {

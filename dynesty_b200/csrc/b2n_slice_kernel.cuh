@@ -44,6 +44,9 @@ struct SliceEval {
         nc++;
         ok = __all_sync(B2N_FULL, ok);          // also orders the writes above
         if (!ok) return -INFINITY;
+#ifdef B2N_USER_PRIOR
+        if (pk == B2N_PRIOR_USER) user_prior_warp(m, &b2n_sm[oun], &b2n_sm[ovn], &b2n_sm[owork], lane);
+#endif
         return loglike_sm<LIKE, PREC_SMEM>(m, ms, Pg, offP, ldP, n, ovn, owork, lane);
     }
 };
@@ -220,6 +223,15 @@ __global__ void __launch_bounds__(512, 1) slice_kernel(const SliceParams p) {
             }
         }
         // v_prop = prior_transform(u_prop) (:1204)
+#ifdef B2N_USER_PRIOR
+        if (pk == B2N_PRIOR_USER) {
+            user_prior_warp(p.m, &b2n_sm[ou], &b2n_sm[ovn], &b2n_sm[owork], lane);
+            for (int i = lane; i < n; i += 32) {
+                peer_put(p.peer, &p.u[(size_t)q * n + i], b2n_sm[ou + i]);
+                peer_put(p.peer, &p.v[(size_t)q * n + i], b2n_sm[ovn + i]);
+            }
+        } else
+#endif
         for (int i = lane; i < n; i += 32) {
             const double ui = b2n_sm[ou + i];
             peer_put(p.peer, &p.u[(size_t)q * n + i], ui);

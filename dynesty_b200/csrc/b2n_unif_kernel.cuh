@@ -120,6 +120,9 @@ __global__ void __launch_bounds__(256) unif_kernel(const UnifParams p) {
             __syncwarp();
             for (int i = lane; i < n; i += 32) vv[i] = prior_1d(p.m, i, uu[i]);
             __syncwarp();
+#ifdef B2N_USER_PRIOR
+            if (p.m.prior_kind == B2N_PRIOR_USER) user_prior_warp(p.m, uu, vv, work, lane);
+#endif
             lcur = warp_loglike<LIKE>(p.m, p.m.lmat, vv, work, lane);
             ncall++;
             if (lcur > loglstar_) done = true;
@@ -185,6 +188,9 @@ __global__ void __launch_bounds__(128) unitcube_kernel(const CubeParams p) {
             }
             g.tick++;
             __syncwarp();
+#ifdef B2N_USER_PRIOR
+            if (p.m.prior_kind == B2N_PRIOR_USER) user_prior_warp(p.m, uu, vv, work, lane);
+#endif
             lcur = warp_loglike<LIKE>(p.m, p.m.lmat, vv, work, lane);
             ncall++;
             if (lcur > loglstar_) break;

@@ -11,8 +11,8 @@ same object can be handed to dynesty's own ``NestedSampler`` as
 (unit-cube warm-up phase, initial live points) while the B200 samplers pick up
 the descriptor for the in-kernel evaluation.
 
-``DeviceModel.from_cuda`` opens the registry: the log-likelihood is then user CUDA code compiled into the same
-kernels at run time (NVRTC, ``usermodel.py``).
+``DeviceModel.from_cuda`` opens the registry: the log-likelihood, and optionally the prior transform, is then user
+CUDA code compiled into the same kernels at run time (NVRTC, ``usermodel.py``).
 """
 import ctypes as C
 import math
@@ -53,8 +53,9 @@ class DeviceModel:
 
     @classmethod
     def from_cuda(cls, ndim, source, params=None, prior_kind=_lib.PRIOR_IDENTITY, prior_p0=None, prior_p1=None,
-                  name='user'):
-        """A model whose log-likelihood is user CUDA code, compiled into the proposal kernels at run time.
+                  prior_source=None, prior_params=None, name='user'):
+        """A model whose log-likelihood (and optionally prior transform) is user CUDA code, compiled into the
+        proposal kernels at run time.
 
         ``source`` defines ONE warp-cooperative device function::
 
@@ -82,15 +83,63 @@ class DeviceModel:
                 return __shfl_sync(0xffffffffu, l, 0);
             }
 
-        The prior is one of the registry's (``prior_kind`` with per-dimension ``prior_p0`` / ``prior_p1``).  The
-        model is accepted wherever a registry model is: every sampler, the device-resident rounds, the dynamic
+        The prior is one of the registry's (``prior_kind`` with per-dimension ``prior_p0`` / ``prior_p1``), or
+        user code: ``prior_source`` defines a second warp-cooperative device function (the prior is then
+        ``PRIOR_USER``)::
+
+            __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane);
+
+        * all 32 lanes call it; it writes ``v[0, n)`` from ``u[0, n)`` and may read ANY component of ``u``, so
+          joint transforms (correlated Gaussians, ordered parameters, simplex weights) are allowed;
+        * ``u``: read only (warp-private shared memory in the chain kernels, global memory in ``evaluate``);
+        * ``v``, ``work``: ``n`` doubles each of warp-private shared memory; ``work`` is undefined on entry;
+        * ``p``: ``prior_params`` (float64) in device memory, or NULL when ``prior_params`` is None;
+        * the caller synchronises the warp before and after the call; inside it, ``__syncwarp()`` between one lane
+          writing ``work`` and another reading it.  The ``b2n_warp_*`` reductions are available;
+        * it must be deterministic (the same ``u`` gives the same bits of ``v``).  Only proposals inside the unit
+          cube are transformed.
+
+        Per dimension -- log-uniform on ``[p[i], p[n + i]]``::
+
+            __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane) {
+                for (int i = lane; i < n; i += 32) v[i] = p[i] * exp(u[i] * log(p[n + i] / p[i]));
+            }
+
+        Joint -- a correlated Gaussian ``mu + L ndtri(u)`` (``mu`` = ``p[0, n)``, lower-triangular ``L``
+        column-major at ``p + n``), with ``ndtri(u)`` staged in ``work``::
+
+            __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane) {
+                for (int i = lane; i < n; i += 32) work[i] = normcdfinv(u[i]);
+                __syncwarp();
+                for (int i = lane; i < n; i += 32) {
+                    double s = p[i];
+                    for (int j = 0; j <= i; j++) s = fma(p[n + (size_t)j * n + i], work[j], s);
+                    v[i] = s;
+                }
+            }
+
+        ``prior_source`` excludes ``prior_kind`` / ``prior_p0`` / ``prior_p1``, and ``prior_params`` needs
+        ``prior_source`` (``ValueError`` otherwise).  ``loglikelihood(v)`` stays prior-free.
+
+        The model is accepted wherever a registry model is: every sampler, the device-resident rounds, the dynamic
         sampler, replicas; random walks run on the warp-per-chain kernel.  The source is compiled with NVRTC for
         sm_90a (once per process, ``usermodel.compile_user``); a compile error raises
-        ``usermodel.UserModelCompileError`` carrying NVRTC's log.  Pickling keeps ``source`` and ``params``.
+        ``usermodel.UserModelCompileError`` carrying NVRTC's log.  Pickling keeps ``source``, ``params``,
+        ``prior_source`` and ``prior_params``.
         """
+        if prior_source is not None:
+            if prior_kind not in (_lib.PRIOR_IDENTITY, _lib.PRIOR_USER) or prior_p0 is not None or prior_p1 is not None:
+                raise ValueError('prior_source defines the prior: prior_kind / prior_p0 / prior_p1 do not apply')
+            prior_kind = _lib.PRIOR_USER
+        elif prior_params is not None:
+            raise ValueError('prior_params are the parameters of a user prior: give prior_source as well')
+        elif prior_kind == _lib.PRIOR_USER:
+            raise ValueError('prior_kind PRIOR_USER needs prior_source')
         m = cls(ndim, prior_kind, _lib.LIKE_USER, prior_p0=prior_p0, prior_p1=prior_p1, name=name)
         m.source = str(source)
         m.params = None if params is None else f64(np.ravel(params))
+        m.prior_source = None if prior_source is None else str(prior_source)
+        m.prior_params = None if prior_params is None else f64(np.ravel(prior_params))
         m.logz_truth = None
         return m
 
@@ -111,12 +160,20 @@ class DeviceModel:
 
     def _create_user(self, ctx, prior_kind, mid):
         from . import usermodel
-        cm = usermodel.compile_user(self.source)
+        prior_source = getattr(self, 'prior_source', None)
+        cm = usermodel.compile_user(self.source, prior_source)
         names = (C.c_char_p * len(cm.lowered))(*[s.encode() for s in cm.lowered])
         prm = self.params
-        ctx.check(ctx.lib.b2n_model_create_user(ctx.h, C.byref(self._desc(prior_kind)), ptr(prm),
-                                                0 if prm is None else prm.size, cm.cubin, len(cm.cubin), names,
-                                                C.byref(mid)))
+        nprm = 0 if prm is None else prm.size
+        if prior_source is None:
+            ctx.check(ctx.lib.b2n_model_create_user(ctx.h, C.byref(self._desc(prior_kind)), ptr(prm), nprm,
+                                                    cm.cubin, len(cm.cubin), names, C.byref(mid)))
+            return
+        # the user prior and the likelihood-only (identity prior) model share the one image
+        pp = self.prior_params if prior_kind == _lib.PRIOR_USER else None
+        ctx.check(ctx.lib.b2n_model_create_user_ex(ctx.h, C.byref(self._desc(prior_kind)), ptr(prm), nprm, ptr(pp),
+                                                   0 if pp is None else pp.size, cm.cubin, len(cm.cubin), names,
+                                                   C.byref(mid)))
 
     def model_id(self, ctx=None):
         return self.ids(ctx)[0]

@@ -119,6 +119,7 @@ double b2n_last_kernel_ms(b2n_ctx* ctx);
 #define B2N_PRIOR_IDENTITY   0  /* v = u                                          */
 #define B2N_PRIOR_UNIFORM    1  /* v = p0[i] + p1[i]*u   (lo, width)               */
 #define B2N_PRIOR_NORMAL_PPF 2  /* v = p0[i] + p1[i]*ndtri(u)  (mu, sigma)         */
+#define B2N_PRIOR_USER       3  /* user CUDA code compiled at run time: b2n_model_create_user_ex below  */
 #define B2N_LIKE_GAUSS_PREC  0  /* -0.5 (v-vec0)^T mat (v-vec0) + s0              */
 #define B2N_LIKE_GAUSS_DIAG  1  /* -0.5 sum vec1[i] (v-vec0)[i]^2 + s0            */
 #define B2N_LIKE_EGGBOX      2  /* (2 + prod cos((2 s0 v - s0)/2))^s1  (tmax, power) */
@@ -177,6 +178,53 @@ int b2n_user_kernel_exprs(const char* const** exprs, int32_t* count);
 int b2n_model_create_user(b2n_ctx* ctx, const b2n_model_desc* desc, const double* params, int64_t nparams,
                           const void* image, size_t image_bytes, const char* const* lowered_names,
                           int32_t* model_id);
+
+/* ---- user priors: a user prior transform compiled into the same kernels ---------------------------------------
+ * Beside b2n_user_loglike the user may write a second warp-cooperative device function,
+ *
+ *     __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane);
+ *
+ *   - all 32 lanes of a warp call it; it writes v[0, n) from u[0, n) and may read ANY component of u, so joint
+ *     (non-separable) transforms are allowed: correlated Gaussians, ordered parameters, simplex weights;
+ *   - u: read only, n doubles behind a generic pointer (warp-private shared memory in the chain kernels, global
+ *     memory in b2n_model_eval);
+ *   - v, work: n doubles each of warp-private shared memory; the contents of work are undefined on entry;
+ *   - p: the prior's own parameter array in device memory (nprior_params doubles of b2n_model_create_user_ex),
+ *     or NULL if none;
+ *   - the caller issues __syncwarp() before and after the call; inside it, __syncwarp() between one lane writing
+ *     work (or v) and another lane reading it.  The b2n_warp_* reductions are available;
+ *   - it must be deterministic: the same u gives the same bits of v.
+ * The prior is applied only to proposals inside the unit cube (a random-walk proposal rejected by the cube test
+ * is never transformed).  A per-dimension example (log-uniform on [p[i], p[n+i]]):
+ *
+ *     __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane) {
+ *         for (int i = lane; i < n; i += 32) v[i] = p[i] * exp(u[i] * log(p[n + i] / p[i]));
+ *     }
+ *
+ * A joint example (correlated Gaussian v = mu + L z, z = ndtri(u), mu = p[0, n), L column-major at p + n):
+ *
+ *     __device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane) {
+ *         for (int i = lane; i < n; i += 32) work[i] = normcdfinv(u[i]);
+ *         __syncwarp();
+ *         for (int i = lane; i < n; i += 32) {
+ *             double s = p[i];
+ *             for (int j = 0; j <= i; j++) s = fma(p[n + (size_t)j * n + i], work[j], s);
+ *             v[i] = s;
+ *         }
+ *     }
+ *
+ * The program is then  #define B2N_USER_PRIOR, #include "b2n_user_kernels.cuh", the prior, the likelihood  (same
+ * options and name expressions as above); B2N_USER_PRIOR also defines the marker b2n_user_prior_abi in the image.
+ *
+ * b2n_model_create_user_ex: b2n_model_create_user with the prior's parameters.
+ *   - desc->prior_kind == B2N_PRIOR_USER: the image must define b2n_user_prior_abi (else B2N_ERR_ARG); prior_params
+ *     (host, nprior_params doubles, may be NULL) are copied to the device; desc->prior_p0 / prior_p1 are ignored.
+ *   - any other prior kind: exactly b2n_model_create_user; nprior_params must be 0.
+ * b2n_model_create and b2n_model_create_user reject B2N_PRIOR_USER. */
+int b2n_model_create_user_ex(b2n_ctx* ctx, const b2n_model_desc* desc, const double* params, int64_t nparams,
+                             const double* prior_params, int64_t nprior_params,
+                             const void* image, size_t image_bytes, const char* const* lowered_names,
+                             int32_t* model_id);
 
 /* ---- ellipsoid membership: MultiEllipsoid.within/overlap/contains
  *      (bounding.py:502-523), Ellipsoid.distance_many/contains (:286-305) ----

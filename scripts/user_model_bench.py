@@ -5,6 +5,9 @@ n = 50, the correlated Gaussian behind U(-5, 5)) timed three ways on the same st
   registry-warp   the same model forced onto the warp-per-chain kernel (B2N_RWALK_IMPL=warp)
   user            the precision-matrix Gaussian restated as user CUDA code (DeviceModel.from_cuda), which always
                   runs on the warp-per-chain kernel
+  user-prior      the same user likelihood with the U(-5, 5) box restated as a user prior (b2n_user_prior): the
+                  prior moves out of the fused per-element proposal loop into one warp call per accepted-cube
+                  proposal; the outputs must equal the user row's bit for bit (same_as_user)
 
 Kernel time per fill from CUDA events around the chain kernel (b2n_set_timing), median of --reps fills after
 --warmup; the card name and power limit are read in the same run.  usage: python scripts/user_model_bench.py"""
@@ -38,6 +41,12 @@ __device__ double b2n_user_loglike(const double* v, double* work, int n, const d
 }
 '''
 
+PRIOR_UNIFORM = r'''
+__device__ void b2n_user_prior(const double* u, double* v, double* work, int n, const double* p, int lane) {
+    for (int i = lane; i < n; i += 32) v[i] = fma(p[n + i], u[i], p[i]);
+}
+'''
+
 
 def card():
     try:
@@ -61,6 +70,9 @@ def main():
     reg = DL.gauss_corr(n, 0.4, 5.0)
     user = DeviceModel.from_cuda(n, PREC, params=np.concatenate([reg.like_vec0, reg.like_mat.T.ravel(), [reg.s[0]]]),
                                  prior_kind=_lib.PRIOR_UNIFORM, prior_p0=-5.0, prior_p1=10.0, name='user_gauss_corr')
+    user_prior = DeviceModel.from_cuda(n, PREC, params=user.params, prior_source=PRIOR_UNIFORM,
+                                       prior_params=np.concatenate([np.full(n, -5.0), np.full(n, 10.0)]),
+                                       name='user_prior_gauss_corr')
     rng = np.random.default_rng(1)
     Cm = np.full((n, n), 0.4)
     np.fill_diagonal(Cm, 1.0)
@@ -74,8 +86,9 @@ def main():
     ctx = _lib.default_context()
     ctx.set_timing(True)
     name, plim = card()
-    res = {}
-    for label, m, env in (('registry', reg, None), ('registry-warp', reg, 'warp'), ('user', user, None)):
+    res, outs = {}, {}
+    for label, m, env in (('registry', reg, None), ('registry-warp', reg, 'warp'), ('user', user, None),
+                          ('user-prior', user_prior, None)):
         if env:
             os.environ['B2N_RWALK_IMPL'] = env
         else:
@@ -83,10 +96,13 @@ def main():
         mid = m.model_id()
         ms = []
         for r in range(a.warmup + a.reps):
-            ops.rwalk_batch(mid, u0, loglstar, 0.5, a.walks, 7, chain0=0)
+            o = ops.rwalk_batch(mid, u0, loglstar, 0.5, a.walks, 7, chain0=0)
+            outs[label] = {k: np.array(o[k]) for k in ('u', 'v', 'logl', 'n_accept')}
             if r >= a.warmup:
                 ms.append(ctx.last_kernel_ms())
         res[label] = dict(ms_per_fill=round(float(np.median(ms)), 4), ms_min=round(float(np.min(ms)), 4))
+    res['user-prior']['same_as_user'] = all(np.array_equal(outs['user'][k], outs['user-prior'][k])
+                                            for k in ('u', 'v', 'logl', 'n_accept'))
     os.environ.pop('B2N_RWALK_IMPL', None)
     print(json.dumps(dict(card=name, power_limit=plim, Q=a.Q, walks=a.walks, n=n, reps=a.reps, results=res)))
 
