@@ -95,6 +95,7 @@ SYMBOLS = {
     'b2n_friends_set': (C.c_int, [_P, _I, _P, _L, _I, _P, _P]),
     'b2n_friends_overlap': (C.c_int, [_P, _P, _L, _I, _P]),
     'b2n_friends_unif_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _P, _P, _P, _P, _P, _P]),
+    'b2n_jitter_runs': (C.c_int, [_P, _P, _P, _L, _P, _D, _I, _I, _U64, _U64, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_bound_set': (C.c_int, [_P, _I, _I, _P, _P, _P, _P]),
     'b2n_rwalk_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _P, _P, _P, _P, _P, _P]),
     'b2n_rslice_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _I, _P, _P, _P, _P, _P, _P, _P]),

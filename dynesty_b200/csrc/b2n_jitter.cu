@@ -1,0 +1,398 @@
+// b2n_jitter.cu -- R prior-volume realisations of one dead-point record (utils.py:1273-1467 jitter_run /
+// compute_integrals, :1932-1997 kld_error of the reference), all in FP64.
+//
+// Random streams (B2N layout, oracle/philox.py; restated in oracle/jitter.py): realisation r is the chain
+// (seed, chain0 + r).  Tick 0 is one uniform vector event over the F samples with nlive_flag set; the e-th of them
+// gets ln t = ln(U_e) / n.  Decreasing stretch s (the reference's _find_decrease) is tick s + 1: nstart_s + 1
+// uniforms, y = -ln U, C = prefix sums of y, and its j-th sample gets ln t = ln(C[k_j] / C[k_{j-1}]) with
+// k_j = samples_n[j] - 1 and k_{-1} = nstart_s.
+//
+// The record is cut into SEGMENTS on the host: pieces of at most TILE samples that are either a run of flagged
+// samples outside every stretch (their t come from tick 0) or a piece of one stretch.  A stretch piece only needs
+// C up to the largest index it reads (k of the sample before it, or nstart), so a long stretch (the add_live tail)
+// splits into pieces that each rescan a prefix of its exponentials.  Nothing R x N is stored unless the full arrays
+// are asked for: the two per-segment passes regenerate ln t from the counter-based stream.
+//
+//   pass 1   (segments x R)  ln t, local prefix of ln t (sum D), local log-sum-exp of the weights (E)
+//   scan 1   (R)             logvol and logz at every segment start, logz[-1]
+//   pass 2   (segments x R)  logvol, logwt, logz per sample; segment sums of the h increments (A), of dh * dlogvol (C)
+//                            and of the KL terms (K); the full arrays when asked for
+//   scan 2   (R)             logzerr[-1], h[-1], kld[-1]; the kld prefix at every segment start
+//   offsets  (segments x R)  adds that prefix to the full kld array (only when it is asked for)
+#include "b2n_device.cuh"
+
+#include <algorithm>
+#include <math.h>
+
+namespace {
+
+constexpr int JT_BLOCK = 256;
+constexpr int JT_TILE = 1024;       // samples per segment
+constexpr int JT_CHUNK = 2048;      // exponentials scanned per step
+
+struct JSeg {
+    int64_t a;       // first sample
+    int32_t len;     // samples
+    int32_t tick;    // 0: flagged samples (tick-0 draws); s + 1: piece of stretch s
+    int64_t kprev;   // stretch piece: the C index its first ratio divides by (= the scan length - 1)
+};
+
+struct JArgs {
+    const double* logl;
+    const double* wref;      // input run's logwt, or NULL (no KL divergence)
+    const int32_t* nlive;    // samples_n
+    const int32_t* aux;      // flagged sample: its element of the tick-0 event; stretch sample: k = samples_n - 1
+    const JSeg* seg;
+    int64_t N, nseg;
+    int R;
+    double zref;
+    uint64_t seed, chain0;
+    double* sD; double* sE; double* sV; double* sZ; double* sA; double* sC; double* sK;   // R x nseg each
+    double* zend;            // R: logz[-1]
+    double* out_logz; double* out_logzerr; double* out_h; double* out_kld;                // R each, may be NULL
+    double* f_logvol; double* f_logwt; double* f_logz; double* f_kld;                     // R x N, may be NULL
+};
+
+__device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
+    if (a == -INFINITY) return b;
+    if (b == -INFINITY) return a;
+    const double m = fmax(a, b);
+    return m + log1p(exp(-fabs(a - b)));
+}
+struct OpSum {
+    __device__ static double id() { return 0.0; }
+    __device__ double operator()(double a, double b) const { return a + b; }
+};
+struct OpLae {
+    __device__ static double id() { return -INFINITY; }
+    __device__ double operator()(double a, double b) const { return lae(a, b); }
+};
+
+// In-place inclusive scan of x[0, n) (shared memory, n <= 8 * blockDim) with a fixed association: thread t owns a
+// contiguous run, then warp shuffles, then the warp totals.  Returns the total (identity for n == 0) to every thread.
+template <class Op>
+__device__ double block_scan(double* x, int n, double* wsum, Op op) {
+    const int t = threadIdx.x, lane = t & 31, w = t >> 5, nw = blockDim.x >> 5;
+    const int ipt = (n + blockDim.x - 1) / blockDim.x;
+    const int i0 = min(t * ipt, n), i1 = min(i0 + ipt, n);
+    double acc = Op::id();
+    for (int i = i0; i < i1; i++) { acc = op(acc, x[i]); x[i] = acc; }
+    double v = acc;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const double u = __shfl_up_sync(B2N_FULL, v, o);
+        if (lane >= o) v = op(u, v);
+    }
+    if (lane == 31) wsum[w] = v;
+    __syncthreads();
+    if (w == 0) {
+        double s = lane < nw ? wsum[lane] : Op::id();
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const double u = __shfl_up_sync(B2N_FULL, s, o);
+            if (lane >= o) s = op(u, s);
+        }
+        if (lane < nw) wsum[lane] = s;
+    }
+    __syncthreads();
+    double ex = __shfl_up_sync(B2N_FULL, v, 1);
+    if (lane == 0) ex = Op::id();
+    if (w > 0) ex = op(wsum[w - 1], ex);
+    if (t > 0)
+        for (int i = i0; i < i1; i++) x[i] = op(ex, x[i]);
+    const double total = wsum[nw - 1];
+    __syncthreads();
+    return total;
+}
+
+// ln t of the segment's samples into lt[0, len)
+__device__ void segment_lnt(const JArgs& A, const JSeg& s, int r, double* lt, double* cap, double* buf, double* wsum) {
+    ChainRng g;
+    g.init(A.seed, A.chain0 + (uint64_t)r);
+    const int L = s.len;
+    if (s.tick == 0) {
+        for (int i = threadIdx.x; i < L; i += blockDim.x)
+            lt[i] = log(rng_uniform_elem(g, A.aux[s.a + i])) / (double)A.nlive[s.a + i];
+        __syncthreads();
+        return;
+    }
+    g.tick = (uint32_t)s.tick;
+    // cap[0] = C[kprev], cap[1 + i] = C[k of sample a + i]
+    double carry = 0.0;
+    for (int64_t c0 = 0; c0 <= s.kprev; c0 += JT_CHUNK) {
+        const int m = (int)min((int64_t)JT_CHUNK, s.kprev + 1 - c0);
+        for (int e = threadIdx.x; e < m; e += blockDim.x) buf[e] = -log(rng_uniform_elem(g, (int)(c0 + e)));
+        __syncthreads();
+        const double tot = block_scan(buf, m, wsum, OpSum());
+        for (int q = threadIdx.x; q <= L; q += blockDim.x) {
+            const int64_t k = q == 0 ? s.kprev : (int64_t)A.aux[s.a + q - 1];
+            if (k >= c0 && k < c0 + m) cap[q] = carry + buf[k - c0];
+        }
+        carry += tot;
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < L; i += blockDim.x) lt[i] = log(cap[i + 1] / cap[i]);
+    __syncthreads();
+}
+
+template <int PASS>
+__global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
+    __shared__ double lt[JT_TILE], pv[JT_TILE], cap[JT_TILE + 1], buf[JT_CHUNK], wsum[32];
+    const int64_t sg = blockIdx.x;
+    const int r = blockIdx.y;
+    const JSeg s = A.seg[sg];
+    const int L = s.len;
+    const int64_t so = (int64_t)r * A.nseg + sg;
+    segment_lnt(A, s, r, lt, cap, buf, wsum);
+    for (int i = threadIdx.x; i < L; i += blockDim.x) pv[i] = lt[i];
+    __syncthreads();
+    const double D = block_scan(pv, L, wsum, OpSum());      // pv[i] = sum of lt[0..i]
+    const double ln_half = -0.69314718055994530942;
+    if (PASS == 1) {
+        for (int i = threadIdx.x; i < L; i += blockDim.x) {
+            const int64_t j = s.a + i;
+            const double lprev = j > 0 ? A.logl[j - 1] : -1e300;
+            buf[i] = (i > 0 ? pv[i - 1] : 0.0) + lae(A.logl[j], lprev) + log1p(-exp(lt[i])) + ln_half;
+        }
+        __syncthreads();
+        const double E = block_scan(buf, L, wsum, OpLae());
+        if (threadIdx.x == 0) { A.sD[so] = D; A.sE[so] = E; }
+        return;
+    }
+    const double V = A.sV[so], Z = A.sZ[so], zmax = A.zend[r];
+    const size_t fo = (size_t)r * A.N + s.a;
+    // logwt (cap), then its log-sum-exp scan (buf) -> logz
+    for (int i = threadIdx.x; i < L; i += blockDim.x) {
+        const int64_t j = s.a + i;
+        const double lprev = j > 0 ? A.logl[j - 1] : -1e300;
+        cap[i] = lae(A.logl[j], lprev) + V + (i > 0 ? pv[i - 1] : 0.0) + log1p(-exp(lt[i])) + ln_half;
+        buf[i] = cap[i];
+    }
+    __syncthreads();
+    block_scan(buf, L, wsum, OpLae());
+    for (int i = threadIdx.x; i < L; i += blockDim.x) buf[i] = lae(Z, buf[i]);
+    __syncthreads();
+    // per sample: the increment a_i of h1 = cumsum(a), dh_i * dlogvol_i, the KL term (read-only pass; thread t owns
+    // samples t + u * blockDim)
+    constexpr int U = JT_TILE / JT_BLOCK;
+    double* sa = buf + JT_TILE;
+    double c_r[U], k_r[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        const int i = threadIdx.x + u * JT_BLOCK;
+        c_r[u] = k_r[u] = 0.0;
+        if (i >= L) continue;
+        const int64_t j = s.a + i;
+        const double l = A.logl[j], lprev = j > 0 ? A.logl[j - 1] : -1e300;
+        const double ldv2 = V + (i > 0 ? pv[i - 1] : 0.0) + log1p(-exp(lt[i])) + ln_half;
+        const double a = exp(l - zmax + ldv2) * l + exp(lprev - zmax + ldv2) * lprev;
+        const double dh = a - zmax * (exp(buf[i] - zmax) - exp((i > 0 ? buf[i - 1] : Z) - zmax));
+        sa[i] = a;
+        c_r[u] = dh * -lt[i];
+        if (A.wref) {
+            const double lp1 = cap[i] - zmax;
+            k_r[u] = exp(lp1) * (lp1 - (A.wref[j] - A.zref));
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < L; i += blockDim.x) {
+        if (A.f_logvol) A.f_logvol[fo + i] = V + pv[i];
+        if (A.f_logwt) A.f_logwt[fo + i] = cap[i];
+        if (A.f_logz) A.f_logz[fo + i] = buf[i];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+        const int i = threadIdx.x + u * JT_BLOCK;
+        if (i < L) { lt[i] = c_r[u]; pv[i] = k_r[u]; }
+    }
+    __syncthreads();
+    const double Asum = block_scan(sa, L, wsum, OpSum());
+    const double Csum = block_scan(lt, L, wsum, OpSum());
+    const double Ksum = block_scan(pv, L, wsum, OpSum());
+    if (A.f_kld)
+        for (int i = threadIdx.x; i < L; i += blockDim.x) A.f_kld[fo + i] = pv[i];
+    if (threadIdx.x == 0) { A.sA[so] = Asum; A.sC[so] = Csum; A.sK[so] = Ksum; }
+}
+
+// One realisation per block: running scans over its segments in chunks of JT_TILE.
+// PASS 1: logvol (sV) and logz (sZ) before every segment, zend = logz[-1].
+// PASS 2: the summaries; the kld prefix before every segment into sK (in place) when the full kld array is wanted.
+template <int PASS>
+__global__ void __launch_bounds__(JT_BLOCK) jitter_scan_kernel(JArgs A) {
+    __shared__ double x[JT_TILE], y[JT_TILE], z[JT_TILE], wsum[32];
+    const int r = blockIdx.x;
+    const int64_t base = (int64_t)r * A.nseg;
+    double c0 = 0.0, c1 = PASS == 1 ? -INFINITY : 0.0, c2 = 0.0;
+    for (int64_t g0 = 0; g0 < A.nseg; g0 += JT_TILE) {
+        const int m = (int)min((int64_t)JT_TILE, A.nseg - g0);
+        if (PASS == 1) {
+            for (int i = threadIdx.x; i < m; i += blockDim.x) x[i] = A.sD[base + g0 + i];
+            __syncthreads();
+            const double td = block_scan(x, m, wsum, OpSum());
+            for (int i = threadIdx.x; i < m; i += blockDim.x) {
+                const double v = i > 0 ? c0 + x[i - 1] : c0;
+                y[i] = v;
+                z[i] = v + A.sE[base + g0 + i];
+            }
+            __syncthreads();
+            const double tz = block_scan(z, m, wsum, OpLae());
+            for (int i = threadIdx.x; i < m; i += blockDim.x) {
+                A.sV[base + g0 + i] = y[i];
+                A.sZ[base + g0 + i] = i > 0 ? lae(c1, z[i - 1]) : c1;
+            }
+            c0 += td;
+            c1 = lae(c1, tz);
+        } else {
+            for (int i = threadIdx.x; i < m; i += blockDim.x) {
+                x[i] = A.sA[base + g0 + i];
+                y[i] = A.sC[base + g0 + i];
+                z[i] = A.sK[base + g0 + i];
+            }
+            __syncthreads();
+            const double ta = block_scan(x, m, wsum, OpSum());
+            const double tc = block_scan(y, m, wsum, OpSum());
+            const double tk = block_scan(z, m, wsum, OpSum());
+            if (A.f_kld)
+                for (int i = threadIdx.x; i < m; i += blockDim.x) A.sK[base + g0 + i] = i > 0 ? c2 + z[i - 1] : c2;
+            c0 += ta;
+            c1 += tc;
+            c2 += tk;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x != 0) return;
+    if (PASS == 1) {
+        A.zend[r] = c1;
+        if (A.out_logz) A.out_logz[r] = c1;
+    } else {
+        const double zmax = A.zend[r];
+        if (A.out_logzerr) A.out_logzerr[r] = sqrt(fabs(c1));       // logzvar = |cumsum(dh * dlogvol)|
+        if (A.out_h) A.out_h[r] = c0 - zmax;                        // h1[-1] - zmax * exp(logz[-1] - zmax)
+        if (A.out_kld) A.out_kld[r] = c2;
+    }
+}
+
+__global__ void __launch_bounds__(JT_BLOCK) jitter_kld_offsets_kernel(JArgs A) {
+    const int64_t sg = blockIdx.x;
+    const int r = blockIdx.y;
+    const JSeg s = A.seg[sg];
+    const double off = A.sK[(int64_t)r * A.nseg + sg];
+    double* f = A.f_kld + (size_t)r * A.N + s.a;
+    for (int i = threadIdx.x; i < s.len; i += blockDim.x) f[i] += off;
+}
+
+// The segment table and the per-sample aux words (the stretch plan; depends on samples_n only).  O(N), one pass.
+int jitter_plan(const int64_t* n, int64_t N, int approx, std::vector<JSeg>& seg, std::vector<int32_t>& aux) {
+    seg.clear();
+    aux.assign(N, 0);
+    int64_t rank = 0;                  // tick-0 elements handed out so far
+    int64_t nstretch = 0;
+    auto dec = [&](int64_t i) { return !approx && i > 0 && i < N && n[i] < n[i - 1]; };
+    JSeg open{0, 0, 0, 0};
+    auto flush = [&]() { if (open.len > 0) seg.push_back(open); open.len = 0; };
+    int64_t i = 0;
+    while (i < N) {
+        if (n[i] < 1 || n[i] > INT32_MAX) return B2N_ERR_ARG;
+        if (dec(i + 1)) {              // sample i opens a decreasing stretch [i, j)
+            flush();
+            int64_t j = i + 1;
+            while (j < N && dec(j)) j++;
+            rank++;                    // the stretch's first sample still takes its tick-0 element
+            const int64_t nstart = n[i];
+            nstretch++;
+            if (nstretch >= (int64_t)UINT32_MAX) return B2N_ERR_ARG;
+            for (int64_t m = i; m < j; m++) {
+                if (n[m] < 1) return B2N_ERR_ARG;
+                aux[m] = (int32_t)(n[m] - 1);
+            }
+            for (int64_t a = i; a < j; a += JT_TILE) {
+                const int64_t kprev = a == i ? nstart : n[a - 1] - 1;
+                seg.push_back(JSeg{a, (int32_t)std::min<int64_t>(JT_TILE, j - a), (int32_t)nstretch, kprev});
+            }
+            i = j;
+            continue;
+        }
+        if (rank > INT32_MAX) return B2N_ERR_ARG;
+        if (open.len == 0) open = JSeg{i, 0, 0, 0};
+        aux[i] = (int32_t)rank++;
+        if (++open.len == JT_TILE) flush();
+        i++;
+    }
+    flush();
+    return B2N_OK;
+}
+
+}  // namespace
+
+extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
+                               const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
+                               uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
+                               double* logvol_full, double* logwt_full, double* logz_full, double* kld_full) {
+    if (!ctx || !logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
+    if (!logwt_ref && (kld || kld_full)) return B2N_ERR_ARG;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    std::vector<JSeg> seg;
+    std::vector<int32_t> aux;
+    B2N_TRY(jitter_plan(samples_n, N, approx, seg, aux));
+    std::vector<int32_t> nl(N);
+    for (int64_t i = 0; i < N; i++) nl[i] = (int32_t)samples_n[i];
+    const int64_t nseg = (int64_t)seg.size();
+    if (nseg > INT32_MAX) return B2N_ERR_ARG;
+
+    JArgs A;
+    memset(&A, 0, sizeof(A));
+    const void* p;
+    B2N_TRY(b2n_in(ctx, ctx->in0, logl, (size_t)N * sizeof(double), &p));
+    A.logl = (const double*)p;
+    B2N_TRY(b2n_in(ctx, ctx->in1, logwt_ref, logwt_ref ? (size_t)N * sizeof(double) : 0, &p));
+    A.wref = (const double*)p;
+    B2N_TRY(b2n_in_host(ctx, ctx->in2, nl.data(), (size_t)N * sizeof(int32_t), &p));
+    A.nlive = (const int32_t*)p;
+    B2N_TRY(b2n_in_host(ctx, ctx->in3, aux.data(), (size_t)N * sizeof(int32_t), &p));
+    A.aux = (const int32_t*)p;
+    B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
+    A.seg = (const JSeg*)p;
+    A.N = N; A.nseg = nseg; A.R = R; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0;
+    // per-(realisation, segment) scratch: 7 x R x nseg, + logz[-1] per realisation
+    const size_t rs = (size_t)R * nseg;
+    B2N_CUDA(ctx, ctx->scratch1.ensure((7 * rs + R) * sizeof(double)));
+    double* sp = ctx->scratch1.as<double>();
+    A.sD = sp; A.sE = sp + rs; A.sV = sp + 2 * rs; A.sZ = sp + 3 * rs;
+    A.sA = sp + 4 * rs; A.sC = sp + 5 * rs; A.sK = sp + 6 * rs; A.zend = sp + 7 * rs;
+    void* d;
+    double* const sum_user[4] = {logz, logzerr, h, kld};
+    double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
+    DevBuf* const sum_buf[4] = {&ctx->out4, &ctx->out5, &ctx->out6, &ctx->out7};
+    for (int k = 0; k < 4; k++) {
+        B2N_TRY(b2n_out(ctx, *sum_buf[k], sum_user[k], (size_t)R * sizeof(double), &d));
+        *sum_dev[k] = (double*)d;
+    }
+    double* const full_user[4] = {logvol_full, logwt_full, logz_full, kld_full};
+    double** const full_dev[4] = {&A.f_logvol, &A.f_logwt, &A.f_logz, &A.f_kld};
+    DevBuf* const full_buf[4] = {&ctx->out0, &ctx->out1, &ctx->out2, &ctx->out3};
+    for (int k = 0; k < 4; k++) {
+        B2N_TRY(b2n_out(ctx, *full_buf[k], full_user[k], (size_t)R * N * sizeof(double), &d));
+        *full_dev[k] = (double*)d;
+    }
+
+    B2N_TIME_BEGIN(ctx);
+    const dim3 grid((unsigned)nseg, (unsigned)R);
+    jitter_pass_kernel<1><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    jitter_scan_kernel<1><<<R, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    jitter_pass_kernel<2><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    jitter_scan_kernel<2><<<R, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    if (A.f_kld) {
+        jitter_kld_offsets_kernel<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+        B2N_LAUNCH_CHECK(ctx);
+    }
+    B2N_TIME_END(ctx);
+
+    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
+    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, full_user[k], *full_dev[k], (size_t)R * N * sizeof(double)));
+    return b2n_finish(ctx);
+}

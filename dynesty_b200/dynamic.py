@@ -8,7 +8,8 @@ SURVEY.md 8(f) row 4.  What is mirrored (reference py/dynesty/dynamicsampler.py,
   sample_batch                        :1228-1466  the batch run: stop at logl_max, then its live points (n = N, N-1, ..)
   combine_runs                        :1467-1608  merge by logl; live count of a merged point = sum of the runs' counts
                                                   where they overlap; ln X recursion ln X -= ln((n+1)/n); integrals
-  run_nested / add_batch              :1610-2050  baseline, then batches until n_effective / maxbatch
+  stopping_function                   :173-297    stop value from n_effective and the jitter scatter of ln Z
+  run_nested / add_batch              :1610-2050  baseline, then batches until the stop value / maxbatch
 
 B200 mapping: the baseline is ``NestedSampler.run_nested(loop='device')``; a batch is (i) ONE chain launch that
 evolves the `nlive_batch` new live points from the selected saved samples (the reference loops `_new_point`
@@ -18,11 +19,17 @@ unmodified ``dynesty.DynamicNestedSampler`` also runs with the B200 bounds / sam
 (tests/test_gpu_dropin.py); this module is the path that keeps the batches' inner loops on the GPU.
 """
 import math
+import warnings
 
 import numpy as np
 
 from . import nested
 from .nested import Results, _integrate
+
+# chain ids of the stopping checks' jitter realisations: check k of a run uses STOP_CHAIN0 + k * 2^32 + r.  The block
+# [3 * 2^61, 2^63) is disjoint from every id a run draws from (proposal chains count from 0, the initial live points
+# are 2^61 + i, the round driver 2^62 + r), so a seeded dynamic run with a stopping check stays reproducible.
+STOP_CHAIN0 = 3 << 61
 
 
 def _logsumexp(a, b=None):
@@ -79,6 +86,47 @@ def n_effective(logwt):
     """utils.py:1012-1030 get_neff_from_logwt (Kish)."""
     w = np.exp(logwt - np.max(logwt))
     return float(w.sum()**2 / (w * w).sum())
+
+
+def stopping_function(results, args=None, seed=None, chain0=0, return_vals=False, ctx=None):
+    """dynamicsampler.py:173-297: stop = pfrac * stop_post + (1 - pfrac) * stop_evid with
+    stop_post = target_n_effective / n_effective and stop_evid = std(ln Z) / evid_thresh, the std over n_mc jitter
+    realisations (``utils.jitter_realisations``, streams (seed, chain0 + r)) or, with n_mc <= 1, logzerr[-1].
+    args (defaults): pfrac 1.0, evid_thresh 0.1, target_n_effective 10000, n_mc 0, error 'jitter', approx True.
+    Returns stop <= 1 [, (stop_post, stop_evid, stop)]."""
+    from . import utils
+    args = args or {}
+    pfrac = args.get('pfrac', 1.0)
+    if not 0. <= pfrac <= 1.:
+        raise ValueError(f"The provided `pfrac` {pfrac} is not between 0. and 1.")
+    evid_thresh = args.get('evid_thresh', 0.1)
+    if pfrac < 1. and evid_thresh < 0.:
+        raise ValueError(f"The provided `evid_thresh` {evid_thresh} is not non-negative even though `pfrac` is {pfrac}.")
+    target_n_effective = args.get('target_n_effective', 10000)
+    if pfrac > 0. and target_n_effective < 0.:
+        raise ValueError(f"The provided `target_n_effective` {target_n_effective} is not non-negative even though "
+                         f"`pfrac` is {pfrac}")
+    n_mc = args.get('n_mc', 0)
+    if n_mc < 0:
+        raise ValueError(f"The number of realizations {n_mc} must be greater or equal to zero.")
+    if 0 < n_mc < 20:
+        warnings.warn("Using a small number of realizations might result in excessively noisy stopping value "
+                      "estimates.")
+    error = args.get('error', 'jitter')
+    if error not in {'jitter', 'resample'}:
+        raise ValueError(f"The chosen `'error'` option {error} is not valid.")
+    approx = args.get('approx', True)
+    if n_mc > 1:
+        if error == 'resample':
+            raise NotImplementedError("error='resample' is not available: see dynesty_b200.utils.kld_error")
+        lnz = utils.jitter_realisations(results, n_mc, utils._seed(seed), chain0=chain0, approx=approx, ctx=ctx)['logz']
+        lnz_std = np.std(lnz)
+    else:
+        lnz_std = results['logzerr'][-1]
+    stop_evid = lnz_std / evid_thresh
+    stop_post = target_n_effective / n_effective(results['logwt'])
+    stop = pfrac * stop_post + (1. - pfrac) * stop_evid
+    return (bool(stop <= 1.), (stop_post, stop_evid, stop)) if return_vals else bool(stop <= 1.)
 
 
 def merge_two(saved, new, logl_min):
@@ -244,19 +292,41 @@ class DynamicNestedSampler:
 
     # ------------------------------------------------------------------ run_nested (:1610-1928)
     def run_nested(self, nlive_init=None, dlogz_init=0.01, nlive_batch=None, wt_kwargs=None, maxbatch=None,
-                   n_effective=None, maxcall=None, round_size=None):
+                   n_effective=None, maxcall=None, round_size=None, stop_kwargs=None):
         """Baseline run, then batches placed by ``weight_function`` until the Kish effective sample size of the merged
-        run reaches `n_effective` (default max(ndim^2, 10000), :1782-1784) or `maxbatch` batches have been added."""
+        run reaches `n_effective` (default max(ndim^2, 10000), :1782-1784) or `maxbatch` batches have been added.
+
+        With `stop_kwargs` (the args of ``stopping_function``; its target_n_effective is `n_effective`, as in the
+        reference, :1785-1794) the run instead stops once the stopping function's value is <= 1, evaluated before
+        every batch (:1865-1880).  Check k draws its jitter realisations from the streams (seed, STOP_CHAIN0 +
+        k * 2^32 + r); the values of every check are kept in ``self.stop_vals``."""
         target = n_effective if n_effective is not None else max(self.ndim * self.ndim, 10000)
         maxbatch = maxbatch if maxbatch is not None else 1 << 30
+        if stop_kwargs is not None:
+            stop_kwargs = dict(stop_kwargs, target_n_effective=target)
+            self.stop_vals = []
         if self.saved is None:
             self.sample_initial(nlive=nlive_init, dlogz=dlogz_init, maxcall=maxcall, round_size=round_size)
         for _ in range(self.batch, maxbatch):
-            if n_effective_of(self.results) >= target or (maxcall is not None and self.ncall >= maxcall):
+            if maxcall is not None and self.ncall >= maxcall:
                 break
+            if stop_kwargs is None:
+                if n_effective_of(self.results) >= target:
+                    break
+            else:
+                stop, vals = stopping_function(self.results, stop_kwargs, seed=self.seed,
+                                               chain0=self.stop_chain0(self.batch), return_vals=True, ctx=self.ctx)
+                self.stop_vals.append(vals)
+                if stop:
+                    break
             self.add_batch(nlive=nlive_batch, wt_kwargs=wt_kwargs, round_size=round_size,
                            maxcall=None if maxcall is None else maxcall - self.ncall)
         return self.results
+
+    @staticmethod
+    def stop_chain0(batch):
+        """first chain id of the stopping check made when `batch` batches have been added"""
+        return STOP_CHAIN0 + (int(batch) << 32)
 
 
 def n_effective_of(res):

@@ -477,3 +477,33 @@ def ns_get_dead(first, count, ndim, ctx=None, positions=True):
 def ns_destroy(ctx=None):
     ctx = _ctx(ctx)
     ctx.check(ctx.lib.b2n_ns_destroy(ctx.h))
+
+
+# ---- run uncertainties (include/b200nest.h, b2n_jitter_runs) ----------------------------------------------
+def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, arrays=False,
+                ctx=None):
+    """R prior-volume realisations of one record (jitter_run / kld_error, utils.py:1317-1408, 1932-1997); realisation
+    r draws from the B2N stream (seed, chain0 + r).  Returns dict(logz, logzerr, h[, kld]) with R values each (the
+    last elements of the realisations' arrays) and, with arrays=True, logvol_arr, logwt_arr, logz_arr[, kld_arr]
+    (R x N).  kld needs the input run's weights: logwt_ref (N) and logz_ref (its logz[-1])."""
+    ctx = _ctx(ctx)
+    logl = f64(logl)
+    n = np.ascontiguousarray(samples_n, dtype=np.int64)
+    N, R = len(logl), int(R)
+    if len(n) != N:
+        raise ValueError("logl and samples_n differ in length")
+    kl = logwt_ref is not None
+    wref = f64(logwt_ref) if kl else None
+    if kl and len(wref) != N:
+        raise ValueError("logwt_ref and logl differ in length")
+    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
+    if kl:
+        o['kld'] = np.empty(R)
+    if arrays:
+        for k in ('logvol', 'logwt', 'logz') + (('kld',) if kl else ()):
+            o[k + '_arr'] = np.empty((R, N))
+    ctx.check(ctx.lib.b2n_jitter_runs(ctx.h, ptr(logl), ptr(n), N, ptr(wref), float(logz_ref) if kl else 0.0,
+                                      int(bool(approx)), R, int(seed), int(chain0), ptr(o['logz']),
+                                      ptr(o['logzerr']), ptr(o['h']), ptr(o.get('kld')), ptr(o.get('logvol_arr')),
+                                      ptr(o.get('logwt_arr')), ptr(o.get('logz_arr')), ptr(o.get('kld_arr'))))
+    return o

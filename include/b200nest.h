@@ -291,6 +291,32 @@ int b2n_bootstrap_expand(b2n_ctx* ctx, const double* points, int64_t N, int32_t 
                          int32_t multi, int32_t nboot, uint64_t seed, uint64_t chain0,
                          double* expands);
 
+/* ---- run uncertainties: prior-volume realisations (utils.py:1273-1467 jitter_run, :1932-1997 kld_error) ------
+ * R realisations of one dead-point record of N samples (logl ascending, samples_n = live points at each sample).
+ * Realisation r draws from the B2N stream (seed, chain0 + r) in the reference's own call order, so the unmodified
+ * reference driven by oracle.jitter.ScriptedJitterGenerator(seed, chain0 + r) consumes the same numbers:
+ *   tick 0      one uniform vector event over the F samples whose nlive_flag is set (_find_decrease, :1273-1314;
+ *               approx != 0: every sample, F = N).  The e-th flagged sample gets ln t = ln(U_e) / samples_n
+ *               (rstate.beta(a=samples_n[flag], b=1), :1368).  A flagged sample that opens a decreasing stretch
+ *               still takes its element; its t is then replaced by the stretch's.
+ *   tick s + 1  decreasing stretch s (samples [b0, b1), nstart = samples_n[b0]): nstart + 1 uniforms, y = -ln U
+ *               (rstate.exponential(size=nstart+1), :1384), C = prefix sums of y; sample b0 + j gets
+ *               ln t = ln(C[k_j] / C[k_{j-1}]), k_j = samples_n[b0 + j] - 1, k_{-1} = nstart (:1385-1389).
+ * Then logvol = cumsum(ln t), the trapezoid integrals of compute_integrals (:1411-1467) give logwt, logz, logzvar
+ * and h, and kld = cumsum(p1 (ln p1 - ln p2)) with ln p1 = logwt - logz[-1], ln p2 = logwt_ref - logz_ref (the
+ * input run's weights, :1976-1992).  logwt_ref NULL: no KL divergence (kld and kld_full must then be NULL).
+ * All arithmetic is FP64; the sums are reassociated (block scans), so values agree with the sequential numpy
+ * formulas to rounding, and realisation r does not depend on R.
+ * samples_n: HOST, N (the stretch plan is built from it on the host).  logl, logwt_ref: N.
+ * Summary outputs, R each, each may be NULL: logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1], kld[-1].
+ * Full outputs, R x N row-major, each may be NULL: logvol, logwt, logz, kld.  Without them no R x N buffer is
+ * allocated.  A fixed number of kernel launches (4, 5 with kld_full), whatever R, N or the number of stretches;
+ * R <= 65535.  Synchronises in host-pointer mode. */
+int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
+                    const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
+                    uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
+                    double* logvol_full, double* logwt_full, double* logz_full, double* kld_full);
+
 /* ---- resident bound for the proposal kernels --------------------------------
  * Uploads K ellipsoids of dimension ncdim (what Sampler ships to every task as
  * `axes` / kwargs['bound'], sampler.py:708-717, internal_samplers.py:229-233).
