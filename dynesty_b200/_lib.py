@@ -122,6 +122,10 @@ SYMBOLS = {
     'b2n_ns_reserve_dead': (C.c_int, [_P, _L]),
     'b2n_ns_get_live': (C.c_int, [_P, _P, _P, _P]),
     'b2n_ns_get_dead': (C.c_int, [_P, _L, _L, _P, _P, _P, _P, _P]),
+    'b2n_ns_get_strands': (C.c_int, [_P, _L, _L, _P, _P]),
+    'b2n_ns_set_live_it': (C.c_int, [_P, _P]),
+    'b2n_ns_get_live_it': (C.c_int, [_P, _P]),
+    'b2n_resample_runs': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

@@ -55,6 +55,9 @@ struct NsDev {
     double *live_u, *live_v, *live_logl;
     double *dead_u, *dead_v, *dead_logl, *dead_logvol;
     int* dead_ncall;
+    int* dead_slot;             // live slot the dead point occupied (its strand)
+    long long* dead_it;         // dead rows recorded before it entered the live set
+    long long* live_it;         // per slot: that count for the slot's current occupant
     NsScalars* sc;
     B2nDyn* dyn;
     int* sidx;          // live rows sorted by (logl, row) ascending -- maintained across rounds
@@ -77,7 +80,7 @@ struct b2n_ns {
     NsDev d;
     long long dead_cap = 0;
     std::vector<void*> allocs;
-    void* dead_alloc[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    void* dead_alloc[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     int phase = 1;                     // host copy of NsScalars::phase (transitions are host-mediated)
     // CUDA graph of B2N_NS_GRAPH_ROUNDS rounds ([commit+propose | chains] x G): every per-round argument of these
     // kernels lives in HBM (B2nDyn, NsScalars), so the launch sequence is STATIC and a block of rounds can be one
@@ -377,6 +380,11 @@ __device__ __forceinline__ void ns_commit_body(const NsDev& s) {
         s.dead_logl[it0 + j] = L;
         s.dead_logvol[it0 + j] = lv;
         s.dead_ncall[it0 + j] = s.o_ncall[j];
+        // strand record: the replacement enters after it0 + K dead rows, i.e. above the round threshold
+        const int slot = cidx[j];
+        s.dead_slot[it0 + j] = slot;
+        s.dead_it[it0 + j] = s.live_it[slot];
+        s.live_it[slot] = it0 + K;
         const double lo = s.o_logl[j];
         s.live_logl[cidx[j]] = lo;
         ncall += s.o_ncall[j];
@@ -530,23 +538,24 @@ static int ns_alloc_dead(b2n_ctx* ctx, b2n_ns* ns, long long cap) {
     // (re)allocate the dead-point arrays with room for `cap` rows, keeping the first `it` rows
     NsDev& d = ns->d;
     const size_t n = d.n;
-    void* nu[5];
-    const size_t bytes[5] = {(size_t)cap * n * 8, (size_t)cap * n * 8, (size_t)cap * 8, (size_t)cap * 8, (size_t)cap * 4};
-    for (int i = 0; i < 5; i++) B2N_CUDA(ctx, cudaMalloc(&nu[i], bytes[i] ? bytes[i] : 8));
+    void* nu[7];
+    const size_t bytes[7] = {(size_t)cap * n * 8, (size_t)cap * n * 8, (size_t)cap * 8, (size_t)cap * 8, (size_t)cap * 4,
+                             (size_t)cap * 4, (size_t)cap * 8};
+    for (int i = 0; i < 7; i++) B2N_CUDA(ctx, cudaMalloc(&nu[i], bytes[i] ? bytes[i] : 8));
     if (ns->dead_alloc[0]) {
         NsScalars h;
         B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         B2N_CUDA(ctx, b2n_copy_sync(ctx, &h, d.sc, sizeof(h), cudaMemcpyDeviceToHost));
         const size_t rows = (size_t)std::min<long long>(h.it, ns->dead_cap);
-        const size_t keep[5] = {rows * n * 8, rows * n * 8, rows * 8, rows * 8, rows * 4};
-        for (int i = 0; i < 5; i++) {
+        const size_t keep[7] = {rows * n * 8, rows * n * 8, rows * 8, rows * 8, rows * 4, rows * 4, rows * 8};
+        for (int i = 0; i < 7; i++) {
             if (keep[i]) B2N_CUDA(ctx, b2n_copy_sync(ctx, nu[i], ns->dead_alloc[i], keep[i], cudaMemcpyDeviceToDevice));
             cudaFree(ns->dead_alloc[i]);
         }
     }
-    for (int i = 0; i < 5; i++) ns->dead_alloc[i] = nu[i];
+    for (int i = 0; i < 7; i++) ns->dead_alloc[i] = nu[i];
     d.dead_u = (double*)nu[0]; d.dead_v = (double*)nu[1]; d.dead_logl = (double*)nu[2];
-    d.dead_logvol = (double*)nu[3]; d.dead_ncall = (int*)nu[4];
+    d.dead_logvol = (double*)nu[3]; d.dead_ncall = (int*)nu[4]; d.dead_slot = (int*)nu[5]; d.dead_it = (long long*)nu[6];
     ns->dead_cap = cap;
     d.dead_cap = cap;
     return B2N_OK;
@@ -661,6 +670,7 @@ int b2n_ns_create(b2n_ctx* ctx, const b2n_ns_config* c, int64_t dead_capacity) {
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.live_u, N * n * 8));
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.live_v, N * n * 8));
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.live_logl, N * 8));
+        B2N_TRY(ns_alloc(ctx, ns, (void**)&d.live_it, N * 8));
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.sc, sizeof(NsScalars)));
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.dyn, sizeof(B2nDyn)));
         B2N_TRY(ns_alloc(ctx, ns, (void**)&d.sidx, N * 4));
@@ -736,6 +746,7 @@ int b2n_ns_set_state(b2n_ctx* ctx, const double* live_u, const double* live_v, c
     // (stream-ordered: a legacy-default-stream memset is NOT ordered against this context's non-blocking stream -- under
     //  load it landed between a proposal and its chain launch and zeroed the round's threshold: round 2, 32 replicas)
     B2N_CUDA(ctx, cudaMemsetAsync(d.dyn, 0, sizeof(B2nDyn), ctx->stream));
+    B2N_CUDA(ctx, cudaMemsetAsync(d.live_it, 0, N * 8, ctx->stream));       // every occupant entered before dead row 0
     const size_t smem = ns_sort_smem(d);
     if (smem > (size_t)ctx->max_smem_optin) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "nlive too large for the one-CTA sort of b2n_ns");
     B2N_TRY(b2n_func_smem(ctx, (const void*)(ns_sort_kernel), (size_t)(smem)));
@@ -1011,6 +1022,38 @@ int b2n_ns_get_dead(b2n_ctx* ctx, int64_t first, int64_t count, double* u, doubl
     if (logl) B2N_CUDA(ctx, b2n_copy_sync(ctx, logl, d.dead_logl + f, c * 8, cudaMemcpyDeviceToHost));
     if (logvol) B2N_CUDA(ctx, b2n_copy_sync(ctx, logvol, d.dead_logvol + f, c * 8, cudaMemcpyDeviceToHost));
     if (ncall) B2N_CUDA(ctx, b2n_copy_sync(ctx, ncall, d.dead_ncall + f, c * 4, cudaMemcpyDeviceToHost));
+    return B2N_OK;
+}
+
+
+int b2n_ns_get_strands(b2n_ctx* ctx, int64_t first, int64_t count, int32_t* slot, int64_t* it) {
+    if (!ctx || !ctx->ns || first < 0 || count < 0) return B2N_ERR_ARG;
+    NsDev& d = ctx->ns->d;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (first + count > ctx->ns->dead_cap) return B2N_ERR_ARG;
+    const size_t f = (size_t)first, c = (size_t)count;
+    if (c == 0) return B2N_OK;
+    if (slot) B2N_CUDA(ctx, b2n_copy_sync(ctx, slot, d.dead_slot + f, c * 4, cudaMemcpyDeviceToHost));
+    if (it) B2N_CUDA(ctx, b2n_copy_sync(ctx, it, d.dead_it + f, c * 8, cudaMemcpyDeviceToHost));
+    return B2N_OK;
+}
+
+int b2n_ns_set_live_it(b2n_ctx* ctx, const int64_t* live_it) {
+    if (!ctx || !ctx->ns || !ctx->ns->active || !live_it) return B2N_ERR_ARG;
+    NsDev& d = ctx->ns->d;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    B2N_CUDA(ctx, b2n_copy_sync(ctx, d.live_it, live_it, (size_t)d.N * 8, cudaMemcpyHostToDevice));
+    return B2N_OK;
+}
+
+int b2n_ns_get_live_it(b2n_ctx* ctx, int64_t* live_it) {
+    if (!ctx || !ctx->ns || !live_it) return B2N_ERR_ARG;
+    NsDev& d = ctx->ns->d;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    B2N_CUDA(ctx, b2n_copy_sync(ctx, live_it, d.live_it, (size_t)d.N * 8, cudaMemcpyDeviceToHost));
     return B2N_OK;
 }
 

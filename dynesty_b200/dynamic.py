@@ -91,7 +91,8 @@ def n_effective(logwt):
 def stopping_function(results, args=None, seed=None, chain0=0, return_vals=False, ctx=None):
     """dynamicsampler.py:173-297: stop = pfrac * stop_post + (1 - pfrac) * stop_evid with
     stop_post = target_n_effective / n_effective and stop_evid = std(ln Z) / evid_thresh, the std over n_mc jitter
-    realisations (``utils.jitter_realisations``, streams (seed, chain0 + r)) or, with n_mc <= 1, logzerr[-1].
+    realisations (``utils.jitter_realisations`` or, with error='resample', ``utils.resample_realisations``; streams
+    (seed, chain0 + r)) or, with n_mc <= 1, logzerr[-1].
     args (defaults): pfrac 1.0, evid_thresh 0.1, target_n_effective 10000, n_mc 0, error 'jitter', approx True.
     Returns stop <= 1 [, (stop_post, stop_evid, stop)]."""
     from . import utils
@@ -118,8 +119,10 @@ def stopping_function(results, args=None, seed=None, chain0=0, return_vals=False
     approx = args.get('approx', True)
     if n_mc > 1:
         if error == 'resample':
-            raise NotImplementedError("error='resample' is not available: see dynesty_b200.utils.kld_error")
-        lnz = utils.jitter_realisations(results, n_mc, utils._seed(seed), chain0=chain0, approx=approx, ctx=ctx)['logz']
+            lnz = utils.resample_realisations(results, n_mc, utils._seed(seed), chain0=chain0, ctx=ctx)['logz']
+        else:
+            lnz = utils.jitter_realisations(results, n_mc, utils._seed(seed), chain0=chain0, approx=approx,
+                                            ctx=ctx)['logz']
         lnz_std = np.std(lnz)
     else:
         lnz_std = results['logzerr'][-1]
@@ -183,16 +186,22 @@ class DynamicNestedSampler:
         self.ncall = 0
         self.batch_bounds = []
         self.results = None
+        self.strands = False              # record samples_id / samples_it (run_nested(strands=True))
 
     def _sampler(self, nlive, seed, live_points=None):
         return nested.NestedSampler(self.model, nlive=nlive, bound=self.bound, sample=self.sample, seed=seed, ctx=self.ctx,
                                     live_points=live_points, **self.kw)
 
     @staticmethod
-    def _record(res, batch_id):
-        return dict(u=res['samples_u'], v=res['samples'], logl=res['logl'], n=np.asarray(res['samples_n'], dtype=np.int64),
-                    nc=np.asarray(res['ncall_per_it'], dtype=np.int64), scale=np.asarray(res['samples_scale'], dtype=float),
-                    batch=np.full(len(res['logl']), batch_id, dtype=np.int64))
+    def _record(res, batch_id, id_offset=0):
+        rec = dict(u=res['samples_u'], v=res['samples'], logl=res['logl'], n=np.asarray(res['samples_n'], dtype=np.int64),
+                   nc=np.asarray(res['ncall_per_it'], dtype=np.int64), scale=np.asarray(res['samples_scale'], dtype=float),
+                   batch=np.full(len(res['logl']), batch_id, dtype=np.int64))
+        if 'samples_id' in res:
+            # a batch's strands are new strands: its slot ids follow the saved ones (dynamicsampler.py:1489)
+            rec.update(id=np.asarray(res['samples_id'], dtype=np.int64) + id_offset,
+                       it=np.asarray(res['samples_it'], dtype=np.int64))
+        return rec
 
     def _results(self):
         rec = self.saved
@@ -202,12 +211,15 @@ class DynamicNestedSampler:
                                logzerr=np.sqrt(logzvar), information=h, samples_n=rec['n'], samples_scale=rec['scale'],
                                ncall_per_it=rec['nc'], samples_batch=rec['batch'], batch_bounds=list(self.batch_bounds),
                                nbatch=self.batch)
+        if 'id' in rec:
+            self.results.update(samples_id=rec['id'], samples_it=rec['it'])
         return self.results
 
     # ------------------------------------------------------------------ baseline (sample_initial, :927-1226)
     def sample_initial(self, nlive=None, dlogz=0.01, maxiter=None, maxcall=None, round_size=None):
         s = self._sampler(nlive or self.nlive0, self.seed)
-        res = s.run_nested(dlogz=dlogz, maxiter=maxiter, maxcall=maxcall, add_live=True, loop='device', batch=round_size)
+        res = s.run_nested(dlogz=dlogz, maxiter=maxiter, maxcall=maxcall, add_live=True, loop='device', batch=round_size,
+                           strands=self.strands)
         self.saved = self._record(res, 0)
         self.ncall = int(res['ncall'])
         self.base_sampler = s
@@ -226,7 +238,7 @@ class DynamicNestedSampler:
             # the batch starts from the prior (:413-461): a fresh run from the unit cube up to logl_max
             bs = self._sampler(nlive, seed)
             out = bs.run_nested(dlogz=dlogz, maxiter=maxiter, maxcall=maxcall, add_live=True, loop='device', batch=round_size,
-                                logl_max=None if not np.isfinite(logl_max) else logl_max)
+                                logl_max=None if not np.isfinite(logl_max) else logl_max, strands=self.strands)
             logl_min = -np.inf
             ncall_new = int(out['ncall'])
         else:
@@ -272,6 +284,8 @@ class DynamicNestedSampler:
             bs.ncall = ncall0
             bs.ncall_at_last_update = 0
             bs.it = 1
+            if self.strands:
+                bs.live_it = np.zeros(nlive, dtype=np.int64)     # the batch's points start its strands
             # join the saved run where it crosses logl_min (:598-606): ln X and ln Z there start the batch's dlogz test
             vol_idx = 0 if not np.isfinite(logl_min) else int(np.argmin(np.abs(saved_logl - logl_min))) + 1
             lv0 = float(saved_logvol[vol_idx - 1]) if vol_idx > 0 else 0.0
@@ -282,7 +296,7 @@ class DynamicNestedSampler:
             e = np.empty((0, self.ndim))
             out = bs._finalize(e, e, np.empty(0), np.empty(0), np.empty(0, dtype=np.int64), dev, True)
             ncall_new = int(bs.ncall)
-        new = self._record(out, self.batch + 1)
+        new = self._record(out, self.batch + 1, int(sv['id'].max()) + 1 if 'id' in sv else 0)
         self.saved = merge_two(self.saved, new, logl_min)
         self.ncall += ncall_new
         self.batch += 1
@@ -292,20 +306,25 @@ class DynamicNestedSampler:
 
     # ------------------------------------------------------------------ run_nested (:1610-1928)
     def run_nested(self, nlive_init=None, dlogz_init=0.01, nlive_batch=None, wt_kwargs=None, maxbatch=None,
-                   n_effective=None, maxcall=None, round_size=None, stop_kwargs=None):
+                   n_effective=None, maxcall=None, round_size=None, stop_kwargs=None, strands=False):
         """Baseline run, then batches placed by ``weight_function`` until the Kish effective sample size of the merged
         run reaches `n_effective` (default max(ndim^2, 10000), :1782-1784) or `maxbatch` batches have been added.
 
         With `stop_kwargs` (the args of ``stopping_function``; its target_n_effective is `n_effective`, as in the
         reference, :1785-1794) the run instead stops once the stopping function's value is <= 1, evaluated before
         every batch (:1865-1880).  Check k draws its jitter realisations from the streams (seed, STOP_CHAIN0 +
-        k * 2^32 + r); the values of every check are kept in ``self.stop_vals``."""
+        k * 2^32 + r); the values of every check are kept in ``self.stop_vals``.
+
+        strands=True records every sample's strand (samples_id / samples_it, see NestedSampler.run_nested); a stop on
+        error='resample' turns it on.  It applies from the baseline on: a sampler whose baseline ran without strands
+        cannot add batches with them."""
         target = n_effective if n_effective is not None else max(self.ndim * self.ndim, 10000)
         maxbatch = maxbatch if maxbatch is not None else 1 << 30
         if stop_kwargs is not None:
             stop_kwargs = dict(stop_kwargs, target_n_effective=target)
             self.stop_vals = []
         if self.saved is None:
+            self.strands = bool(strands or (stop_kwargs is not None and stop_kwargs.get('error') == 'resample'))
             self.sample_initial(nlive=nlive_init, dlogz=dlogz_init, maxcall=maxcall, round_size=round_size)
         for _ in range(self.batch, maxbatch):
             if maxcall is not None and self.ncall >= maxcall:

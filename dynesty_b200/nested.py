@@ -182,6 +182,8 @@ class NestedSampler:
         self.bound_history = []           # (ncall, nells, logvol) per update
         self._q = None
         self._qpos = 0
+        self.live_it = None               # strands recorded (run_nested(strands=True)): per slot, the dead points
+                                          # of the run recorded before its occupant entered the live set
 
     # ------------------------------------------------------------------ save / restore (utils.py:2321-2355)
     def __getstate__(self):
@@ -359,12 +361,15 @@ class NestedSampler:
         c.resident_key = m.version                     # these very ellipsoids ARE the resident bound
 
     def _device_rounds(self, logz, logvol, loglstar, dlogz, maxiter, maxcall, batch, checkpoint_file=None,
-                       checkpoint_every=0.0, snap=None, on_checkpoint=None, keep_samples=True, logl_max=None):
+                       checkpoint_every=0.0, snap=None, on_checkpoint=None, keep_samples=True, logl_max=None,
+                       strand_offset=0):
         """Run (or continue) with ``b2n_ns_run`` (include/b200nest.h): K-worst replacement rounds paced on the
         device -- first with prior draws (the phase before the first bound, sampler.py:407-409), then with the
         inner sampler against the resident bound.  The host only reacts to the device's flags: (re)build the bound
         (update_bound, sampler.py:493-510 -- on the device when ``_device_bound_ok``), grow the dead buffer, and
-        collect the dead points at the end."""
+        collect the dead points at the end.  With strands recorded (``self.live_it`` set) the device rounds record
+        every dead point's slot and birth count too (b2n_ns_get_strands); `strand_offset` is the number of dead points
+        of this run recorded before the device phase.  They are left in ``self._dev_strands``."""
         from . import ops
         import time
         n, N = self.ndim, self.nlive
@@ -379,6 +384,8 @@ class NestedSampler:
         K = int(batch or max(1, N // (40 if kind == 0 else 10)))
         self.batch = K
         prev = [np.empty((0, n)), np.empty((0, n)), np.empty(0), np.empty(0), np.empty(0, dtype=np.int32)]
+        strands = self.live_it is not None
+        prev_str = [np.empty(0, dtype=np.int64), np.empty(0, dtype=np.int64)]
         chain_base = self.chain_counter
         it0_orig = it0 = self.it         # iterations before the device phase (enters the efficiency test)
         if snap is not None:             # resume: rows that died before the snapshot, scalars of the run
@@ -389,6 +396,10 @@ class NestedSampler:
             maxiter = maxiter - len(prev[2]) if maxiter < (1 << 61) else maxiter
             it0_orig = snap['it0']
             it0 = it0_orig + len(prev[2])
+            if strands:
+                prev_str, self.live_it = list(snap['strands']), snap['live_it'].copy()
+        # device row 0 is dead point `off` of the run (the device counts strand births from its row 0)
+        off = strand_offset + len(prev[2])
         no_bound = self.bound_next is None
         multi = not isinstance(self.bound_next, B.B200Ellipsoid)
         ops.ns_create(self.model.model_id(self.ctx), N, n, K, kind, steps, self.seed, chain0=chain_base,
@@ -405,6 +416,8 @@ class NestedSampler:
         try:
             ops.ns_set_state(self.live_u, self.live_v, self.live_logl, logvol, logz, loglstar, self.ncall, smp.scale,
                              ctx=self.ctx)
+            if strands:
+                ops.ns_set_live_it(self.live_it - off, ctx=self.ctx)
             rounds0 = 0
             if snap is not None:
                 rounds0 = snap['rounds']
@@ -416,12 +429,18 @@ class NestedSampler:
             t_ckpt, n_ckpt, saved_it = time.perf_counter(), 0, 0
             dev_nells = 0
 
+            def get_strands(st):
+                slot, it = ops.ns_get_strands(saved_it, st['it'] - saved_it, ctx=self.ctx)
+                return [np.concatenate([prev_str[0], slot.astype(np.int64)]), np.concatenate([prev_str[1], it + off])]
+
             def checkpoint(st):
                 """Snapshot at a consistent point (flags clear, bound current): live set, scalars, the rows that
                 died since the last snapshot; then pickle the whole sampler (host phase results included)."""
-                nonlocal saved_it, prev
+                nonlocal saved_it, prev, prev_str
                 new = ops.ns_get_dead(saved_it, st['it'] - saved_it, n, ctx=self.ctx)
                 prev = [np.concatenate([a, b]) for a, b in zip(prev, new)]
+                if strands:
+                    prev_str = get_strands(st)
                 saved_it = st['it']
                 if dev_nells:
                     self._pull_device_bound(dev_nells)
@@ -429,6 +448,8 @@ class NestedSampler:
                                       logz=st['logz'], loglstar=st['loglstar'], ncall=st['ncall'], scale=st['scale'],
                                       rounds=st['rounds'], ncall_last_update=st['ncall_last_update'],
                                       doubling=st['doubling'], chain_base=chain_base, batch=K, it0=it0_orig)
+                if strands:
+                    self._dev_snap.update(strands=prev_str, live_it=ops.ns_get_live_it(N, ctx=self.ctx) + off)
                 self.save(checkpoint_file)
 
             while True:
@@ -494,6 +515,9 @@ class NestedSampler:
             self.live_u, self.live_v, self.live_logl = ops.ns_get_live(N, n, ctx=self.ctx)
             new = ops.ns_get_dead(saved_it, st['it'] - saved_it, n, ctx=self.ctx, positions=keep_samples)
             out = tuple(np.concatenate([a, b]) for a, b in zip(prev, new))
+            if strands:
+                self._dev_strands = tuple(get_strands(st))
+                self.live_it = ops.ns_get_live_it(N, ctx=self.ctx) + off
             self.chain_counter = chain_base + rounds * K
             self.nbatches += rounds - (snap['rounds'] if snap is not None else 0)
             self.n_proposals += self.ncall - ncall_start
@@ -507,7 +531,7 @@ class NestedSampler:
     # ------------------------------------------------------------------ main loop
     def run_nested(self, dlogz=None, maxiter=None, maxcall=None, add_live=True, loop='host', batch=None,
                    checkpoint_file=None, checkpoint_every=60., resume=False, on_checkpoint=None, device_init=True,
-                   keep_samples=True, logl_max=None):
+                   keep_samples=True, logl_max=None, strands=False):
         """sampler.py:1214-1356 / 1040-1212 (no plateau mode: continuous likelihoods).
 
         loop='host'   : the reference's semantics -- one worst point per iteration, replacements
@@ -525,7 +549,11 @@ class NestedSampler:
                         device (results.samples / samples_u are then empty; logz, logzerr, logl, logvol, logwt and the
                         call counts are complete): for ensembles that only want evidences.
         device_init   : False = the phase before the first bound runs in the host loop (queue of prior draws
-                        evaluated on the GPU) and the device takes over when the first bound exists."""
+                        evaluated on the GPU) and the device takes over when the first bound exists.
+        strands       : True = record every sample's strand (the reference's samples_id / samples_it): the results
+                        then carry samples_id, the live slot the point occupied, and samples_it, the number of dead
+                        points of the run recorded before it entered the live set; resample_run and unravel_run
+                        (dynesty_b200.utils) need them."""
         if resume:
             return self._resume(checkpoint_file, checkpoint_every)
         if loop not in ('host', 'device'):
@@ -552,6 +580,9 @@ class NestedSampler:
         dead_v = np.empty((cap, self.ndim))
         dead_l = np.empty(cap)
         dead_nc = np.empty(cap, dtype=np.int64)
+        self.live_it = np.zeros(nlive, dtype=np.int64) if strands else None
+        dead_id = np.empty(cap if strands else 0, dtype=np.int64)
+        dead_it = np.empty(cap if strands else 0, dtype=np.int64)
         ndead = 0
         ncall0 = self.ncall
         hand_over = False
@@ -595,6 +626,11 @@ class NestedSampler:
                 dead_v = np.resize(dead_v, (cap, self.ndim))
                 dead_l = np.resize(dead_l, cap)
                 dead_nc = np.resize(dead_nc, cap)
+                if strands:
+                    dead_id, dead_it = np.resize(dead_id, cap), np.resize(dead_it, cap)
+            if strands:
+                dead_id[ndead], dead_it[ndead] = worst, self.live_it[worst]
+                self.live_it[worst] = ndead + 1                    # enters above this dead point
             dead_u[ndead] = self.live_u[worst]
             dead_v[ndead] = self.live_v[worst]
             dead_l[ndead] = lnew
@@ -613,18 +649,22 @@ class NestedSampler:
         logl = dead_l[:ndead]
         logvols = -dlv * np.arange(1, ndead + 1)
         su, sv, nc_all = dead_u[:ndead], dead_v[:ndead], dead_nc[:ndead]
+        host_str = (dead_id[:ndead].copy(), dead_it[:ndead].copy()) if strands else None
         if hand_over:
             # (kept on the object so that a checkpoint of the device phase carries the host phase's results)
             self._host_part = dict(su=su.copy(), sv=sv.copy(), logl=logl.copy(), logvols=logvols, nc_all=nc_all.copy(),
                                    logz=logz, logvol=logvol, loglstar=loglstar, dlogz=dlogz, add_live=add_live,
                                    maxiter=maxiter - ndead,
                                    maxcall=ncall0 + maxcall if maxcall < (1 << 61) else None)
+            if strands:
+                self._host_part['strands'] = host_str
             dev = self._device_rounds(logz, logvol, loglstar, dlogz, self._host_part['maxiter'],
                                       self._host_part['maxcall'], batch, checkpoint_file=checkpoint_file,
                                       checkpoint_every=checkpoint_every, on_checkpoint=on_checkpoint,
-                                      keep_samples=keep_samples or checkpoint_file is not None, logl_max=logl_max)
-            return self._finalize(su, sv, logl, logvols, nc_all, dev, add_live)
-        return self._finalize(su, sv, logl, logvols, nc_all, None, add_live)
+                                      keep_samples=keep_samples or checkpoint_file is not None, logl_max=logl_max,
+                                      strand_offset=ndead)
+            return self._finalize(su, sv, logl, logvols, nc_all, dev, add_live, host_str)
+        return self._finalize(su, sv, logl, logvols, nc_all, None, add_live, host_str)
 
     def _resume(self, checkpoint_file, checkpoint_every):
         """Continue a run restored from a checkpoint of the device phase (``NestedSampler.restore``)."""
@@ -633,11 +673,13 @@ class NestedSampler:
             raise ValueError("nothing to resume: the pickle carries no snapshot of a device-resident run")
         dev = self._device_rounds(hp['logz'], hp['logvol'], hp['loglstar'], hp['dlogz'], hp['maxiter'], hp['maxcall'],
                                   snap['batch'], checkpoint_file=checkpoint_file, checkpoint_every=checkpoint_every,
-                                  snap=snap)
-        return self._finalize(hp['su'], hp['sv'], hp['logl'], hp['logvols'], hp['nc_all'], dev, hp['add_live'])
+                                  snap=snap, strand_offset=len(hp['logl']))
+        return self._finalize(hp['su'], hp['sv'], hp['logl'], hp['logvols'], hp['nc_all'], dev, hp['add_live'],
+                              hp.get('strands'))
 
-    def _finalize(self, su, sv, logl, logvols, nc_all, dev, add_live):
-        """Results (+ remaining live points, sampler.py:780-914) from the host-phase and device-phase dead points."""
+    def _finalize(self, su, sv, logl, logvols, nc_all, dev, add_live, strands=None):
+        """Results (+ remaining live points, sampler.py:780-914) from the host-phase and device-phase dead points.
+        With strands recorded: `strands` = (samples_id, samples_it) of the host-phase dead points."""
         nlive = self.nlive
         ndead = len(logl)
         have_pos = True
@@ -676,4 +718,11 @@ class NestedSampler:
                                samples_n=samples_n, samples_scale=sample_scale,
                                nbound=self.nbound, nbatches=self.nbatches, n_proposals=self.n_proposals,
                                bound_history=list(self.bound_history), scale_history=list(self.scale_history))
+        if self.live_it is not None:
+            ids, its = strands if strands is not None else (np.empty(0, dtype=np.int64), np.empty(0, dtype=np.int64))
+            if dev is not None:
+                ids, its = np.concatenate([ids, self._dev_strands[0]]), np.concatenate([its, self._dev_strands[1]])
+            if add_live:
+                ids, its = np.concatenate([ids, order]), np.concatenate([its, self.live_it[order]])
+            self.results.update(samples_id=ids.astype(np.int64), samples_it=its.astype(np.int64))
         return self.results

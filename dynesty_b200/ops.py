@@ -474,6 +474,30 @@ def ns_get_dead(first, count, ndim, ctx=None, positions=True):
     return u, v, l, lv, nc
 
 
+def ns_get_strands(first, count, ctx=None):
+    """(slot, it) of dead points [first, first + count): the live slot each occupied (int32) and the dead rows of the
+    device buffer recorded before it entered the live set (int64)."""
+    ctx = _ctx(ctx)
+    slot, it = np.empty(count, dtype=np.int32), np.empty(count, dtype=np.int64)
+    ctx.check(ctx.lib.b2n_ns_get_strands(ctx.h, int(first), int(count), ptr(slot), ptr(it)))
+    return slot, it
+
+
+def ns_set_live_it(live_it, ctx=None):
+    """Per live slot: the dead rows of the device buffer recorded before its occupant entered (negative: before the
+    first row).  Follows ns_set_state, which sets them all to 0."""
+    ctx = _ctx(ctx)
+    a = np.ascontiguousarray(live_it, dtype=np.int64)
+    ctx.check(ctx.lib.b2n_ns_set_live_it(ctx.h, ptr(a)))
+
+
+def ns_get_live_it(nlive, ctx=None):
+    ctx = _ctx(ctx)
+    a = np.empty(int(nlive), dtype=np.int64)
+    ctx.check(ctx.lib.b2n_ns_get_live_it(ctx.h, ptr(a)))
+    return a
+
+
 def ns_destroy(ctx=None):
     ctx = _ctx(ctx)
     ctx.check(ctx.lib.b2n_ns_destroy(ctx.h))
@@ -506,4 +530,42 @@ def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None
                                       int(bool(approx)), R, int(seed), int(chain0), ptr(o['logz']),
                                       ptr(o['logzerr']), ptr(o['h']), ptr(o.get('kld')), ptr(o.get('logvol_arr')),
                                       ptr(o.get('logwt_arr')), ptr(o.get('logz_arr')), ptr(o.get('kld_arr'))))
+    return o
+
+
+def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, chain0=0, logwt_ref=None, logz_ref=None,
+                  multiplicities=False, ctx=None):
+    """R bootstrap realisations of one strand-labelled record (resample_run / kld_error(error='resample'),
+    utils.py:1495-1660, 1932-1997); realisation r draws from the B2N stream (seed, chain0 + r).  strand: compacted
+    strand index per sample (0..S-1); base: per strand, drawn in the base event; piece_ptr / piece_strand: CSR of
+    the pieces whose first covered sample is i; end: per sample, the copies of a final live point share out its live
+    count (or None).  Returns dict(logz, logzerr, h[, kld]) with R values each and, with multiplicities=True, mult
+    (R x S, int64): the times every strand is drawn."""
+    ctx = _ctx(ctx)
+    logl = f64(logl)
+    N = len(logl)
+    strand = np.ascontiguousarray(strand, dtype=np.int32)
+    base = np.ascontiguousarray(base, dtype=np.uint8)
+    pp = np.ascontiguousarray(piece_ptr, dtype=np.int64)
+    ps = np.ascontiguousarray(piece_strand, dtype=np.int32)
+    if len(strand) != N or len(pp) != N + 1:
+        raise ValueError("logl, strand and piece_ptr differ in length")
+    if end is not None:
+        end = np.ascontiguousarray(end, dtype=np.uint8)
+        if len(end) != N:
+            raise ValueError("logl and end differ in length")
+    S, R = len(base), int(R)
+    kl = logwt_ref is not None
+    wref = f64(logwt_ref) if kl else None
+    if kl and len(wref) != N:
+        raise ValueError("logwt_ref and logl differ in length")
+    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
+    if kl:
+        o['kld'] = np.empty(R)
+    m = np.empty((R, S), dtype=np.int32) if multiplicities else None
+    ctx.check(ctx.lib.b2n_resample_runs(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps), ptr(end),
+                                        ptr(wref), float(logz_ref) if kl else 0.0, R, int(seed), int(chain0),
+                                        ptr(o['logz']), ptr(o['logzerr']), ptr(o['h']), ptr(o.get('kld')), ptr(m)))
+    if multiplicities:
+        o['mult'] = m.astype(np.int64)
     return o

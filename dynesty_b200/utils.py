@@ -1,19 +1,25 @@
-"""Run uncertainties from simulated prior volumes, computed on the GPU.
+"""Run uncertainties from simulated prior volumes and from bootstrapped strands, computed on the GPU.
 
 What is mirrored (reference py/dynesty/utils.py, same names / meaning):
-  jitter_run   :1317-1408   one realisation of the prior volumes of a run's dead points
-  kld_error    :1932-1997   the KL divergence from the run to such a realisation
-and ``jitter_realisations``, the batched form the dynamic sampler's stopping function needs: n_mc realisations in one
-call (``b2n_jitter_runs``, a fixed number of kernel launches whatever n_mc, the record length or its number of
-decreasing stretches).
+  jitter_run    :1317-1408   one realisation of the prior volumes of a run's dead points
+  resample_run  :1495-1660   one bootstrap realisation of a run's strands (the points that occupied one live slot)
+  unravel_run   :1711-1814   a run split into its strands
+  kld_error     :1932-1997   the KL divergence from the run to such a realisation
+and the batched forms the dynamic sampler's stopping function needs: ``jitter_realisations`` (``b2n_jitter_runs``) and
+``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches.
 
-Randomness: realisation r of a call is the B2N Philox stream (seed, chain0 + r) (include/b200nest.h,
-b2n_jitter_runs), so a (seed, chain) pair names one realisation: it is the same whether it is computed alone or in a
-batch of any size.  ``seed=None`` draws a fresh seed, like the reference's ``rstate=None``.
+Randomness: realisation r of a call is the B2N Philox stream (seed, chain0 + r) (include/b200nest.h), so a (seed,
+chain) pair names one realisation: it is the same whether it is computed alone or in a batch of any size.
+``seed=None`` draws a fresh seed, like the reference's ``rstate=None``.
 
-``resample_run`` (bootstrap over the threads of a run) is not provided: it needs, for every dead point, the live slot it
-came from (the reference's samples_id / samples_it), and the device rounds do not record that.
+Strands need a record with samples_id / samples_it (``run_nested(strands=True)``).  The live count of a resampled
+point follows the strand rule of include/b200nest.h (b2n_resample_runs, DESIGN.md section 15): every point is live
+from the threshold it entered above to its own logl.  For runs that remove one point at a time this is the
+reference's rule; for the device rounds, which remove `batch` points at once, it keeps the run's own live counts
+where the reference's rule would count every slot as occupied.
 """
+import math
+
 import numpy as np
 
 from . import ops
@@ -67,12 +73,166 @@ def jitter_run(res, seed=None, chain=0, approx=False, ctx=None):
 
 def kld_error(res, error='jitter', seed=None, chain=0, return_new=False, approx=False, ctx=None):
     """kld_error (utils.py:1932-1997): the cumulative KL divergence from `res` to the realisation (seed, chain) of
-    jitter_run; with return_new, also that realisation."""
+    jitter_run (error='jitter') or of resample_run (error='resample'); with return_new, also that realisation."""
     if error == 'resample':
-        raise NotImplementedError(
-            "error='resample' needs resample_run, which needs the live slot every dead point came from (samples_id / "
-            "samples_it); the device rounds do not record it.  Use error='jitter'.")
+        new, idx = resample_run(res, seed, chain, return_idx=True, ctx=ctx)
+        logp2 = (np.asarray(res['logwt']) - np.asarray(res['logz'])[-1])[idx]
+        logp1 = new['logwt'] - new['logz'][-1]
+        kld = np.cumsum(np.exp(logp1) * (logp1 - logp2))
+        return (kld, new) if return_new else kld
     if error != 'jitter':
         raise ValueError("Input `'error'` option '{}' is not valid.".format(error))
     new, kld = _realisation(res, seed, chain, approx, ctx)
     return (kld, new) if return_new else kld
+
+
+# ---------------------------------------------------------------------------------------------- strands
+def strand_plan(res):
+    """The strands of a record and the thresholds its points entered above.  Returns dict(
+      ids      the distinct samples_id (strand s is ids[s]),
+      strand   per sample, its strand s,
+      base     per strand, True if one of its samples is in a batch whose lower bound is -inf (utils.py:1563-1570),
+      birth    per sample, the threshold it entered the live set above: the lower bound of its batch if samples_it
+               is 0, else the logl of its batch's (samples_it - 1)-th sample in record order,
+      start    per sample, the first sample its piece covers: the one after that (samples_it - 1)-th sample, or the
+               first whose logl is above the lower bound (positions, so that equal logl values keep the run's order),
+      end      per sample, True at a strand's last sample when the record ends with its final live points, else None,
+      open     per strand, the first sample covered by its live point that the record does not hold (no final live
+               points: the one after the last point of the round its last recorded point died in), else None)."""
+    if 'samples_id' not in res or 'samples_it' not in res:
+        raise NotImplementedError("error='resample' / resample_run need every sample's strand (samples_id / "
+                                  "samples_it): run the sampler with run_nested(strands=True).")
+    logl = np.asarray(res['logl'], dtype=float)
+    N = len(logl)
+    ids, strand = np.unique(np.asarray(res['samples_id']), return_inverse=True)
+    sit = np.asarray(res['samples_it'], dtype=np.int64)
+    if 'samples_batch' in res:                      # a dynamic record: every batch ends with its live points
+        batch = np.asarray(res['samples_batch'], dtype=np.int64)
+        lower = np.array([b[0] for b in res['batch_bounds']], dtype=float)
+        final_live = True
+    else:
+        batch, lower = np.zeros(N, dtype=np.int64), np.array([-np.inf])
+        final_live = N > int(res['niter'])
+    S = len(ids)
+    base = np.zeros(S, dtype=bool)
+    base[strand[lower[batch] == -np.inf]] = True
+    # the k-th sample of batch b in record order is rec_pos[first[b] + k]
+    rec_pos = np.argsort(batch, kind='stable')
+    cnt = np.bincount(batch, minlength=len(lower))
+    first = np.cumsum(cnt) - cnt
+    birth = lower[batch].copy()
+    start = np.searchsorted(logl, birth, side='right')
+    later = sit > 0
+    prev = rec_pos[first[batch[later]] + sit[later] - 1]
+    birth[later] = logl[prev]
+    start[later] = prev + 1
+    last = np.full(S, -1, dtype=np.int64)
+    np.maximum.at(last, strand, np.arange(N))
+    end = opened = None
+    if final_live:
+        end = np.zeros(N, dtype=bool)
+        end[last] = True
+    else:
+        # a round ends where the live count stops falling (samples_n: nlive in a host loop, N - j in device rounds);
+        # its threshold is the logl of its last point
+        n = np.asarray(res['samples_n'], dtype=np.int64)
+        stops = np.nonzero(np.r_[n[1:] >= n[:-1], True])[0]
+        opened = stops[np.searchsorted(stops, last)] + 1
+    return dict(ids=ids, strand=strand.astype(np.int64), base=base, birth=birth, start=np.minimum(start, np.arange(N)),
+                end=end, open=opened)
+
+
+def _pieces(logl, plan):
+    """Every piece's first covered sample (the first whose logl is above its birth) and its strand: one per sample,
+    then one per strand whose unrecorded live point covers samples of the record."""
+    start, pstr = plan['start'], plan['strand']
+    if plan['open'] is not None:
+        keep = plan['open'] < len(logl)
+        start, pstr = np.r_[start, plan['open'][keep]], np.r_[pstr, np.nonzero(keep)[0]]
+    return start, pstr
+
+
+def _piece_csr(logl, plan):
+    """(piece_ptr, piece_strand) as b2n_resample_runs takes them: the pieces by their first covered sample."""
+    start, pstr = _pieces(logl, plan)
+    ptr_ = np.zeros(len(logl) + 1, dtype=np.int64)
+    ptr_[1:] = np.cumsum(np.bincount(start, minlength=len(logl)))
+    return ptr_, pstr[np.argsort(start, kind='stable')]
+
+
+def resample_realisations(res, n_mc, seed, chain0=0, multiplicities=False, ctx=None):
+    """n_mc resample_run realisations of `res` in one call.  Returns dict(logz, logzerr, h, kld): the last element of
+    each realisation's logz / logzerr / information / cumulative KL divergence (n_mc values each); with
+    multiplicities=True also mult (n_mc x nstrands): the times each strand (in the order of np.unique(samples_id)) is
+    drawn.  Realisation r uses the stream (seed, chain0 + r)."""
+    plan = strand_plan(res)
+    if not plan['base'].any():
+        raise ValueError("The provided `Results` does not include any points initially sampled from the prior!")
+    logl = np.asarray(res['logl'], dtype=float)
+    pptr, pstr = _piece_csr(logl, plan)
+    return ops.resample_runs(logl, plan['strand'], plan['base'], pptr, pstr, plan['end'], int(n_mc), int(seed),
+                             chain0=int(chain0), logwt_ref=res['logwt'], logz_ref=float(np.asarray(res['logz'])[-1]),
+                             multiplicities=multiplicities, ctx=ctx)
+
+
+def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
+    """resample_run (utils.py:1495-1660): a copy of `res` made of a bootstrap draw of its strands -- base strands
+    (started from the prior) drawn with replacement among themselves, add-on strands (started inside a dynamic
+    batch) among themselves -- with the live counts of the strand rule and the integrals of those.  The draw is the
+    stream (seed, chain) (b2n_resample_runs computes it and the summaries; the arrays are built here).  With
+    return_idx, also the index in `res` of every sample of the new run."""
+    plan = strand_plan(res)
+    o = resample_realisations(res, 1, _seed(seed), chain, multiplicities=True, ctx=ctx)
+    m = o['mult'][0]
+    logl = np.asarray(res['logl'], dtype=float)
+    N = len(logl)
+    start, pstr = _pieces(logl, plan)
+    ms = m[plan['strand']]
+    # live count: the pieces covering each sample, weighted by the multiplicity of their strand
+    diff = np.bincount(start, weights=m[pstr], minlength=N)
+    diff[1:] -= ms[:-1]
+    n = np.rint(np.cumsum(diff)).astype(np.int64)
+    idx = np.repeat(np.arange(N), ms)
+    copy = np.arange(len(idx)) - np.repeat(np.cumsum(ms) - ms, ms)
+    samp_n = n[idx] - (0 if plan['end'] is None else copy * plan['end'][idx])     # a final live point's copies
+    logvol = np.cumsum(np.log(samp_n / (samp_n + 1.)))
+    lnew = logl[idx]
+    logwt, logz, logzvar, h = _integrate(lnew, logvol)
+    new = Results(res)
+    nc = np.asarray(res['ncall_per_it'])[idx]
+    new.update(niter=len(idx), ncall_per_it=nc, eff=100. * len(idx) / max(int(nc.sum()), 1), logl=lnew,
+               samples_n=samp_n, logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(np.maximum(logzvar, 0)),
+               information=h)
+    for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'samples_scale'):
+        if k in res and len(res[k]) == N:
+            new[k] = np.asarray(res[k])[idx]
+    return (new, idx) if return_idx else new
+
+
+def unravel_run(res):
+    """unravel_run (utils.py:1711-1814): the run split into its strands, each a run with one live point (host only).
+    Their volumes are those of a one-point run: valid only for strands that started from the prior."""
+    plan = strand_plan(res)
+    ids = np.asarray(res['samples_id'])
+    added_live = plan['end'] is not None
+    logl_all = np.asarray(res['logl'], dtype=float)
+    out = []
+    for s in plan['ids']:
+        sel = ids == s
+        logl = logl_all[sel]
+        nsamps = len(logl)
+        niter = nsamps - 1 if added_live else nsamps
+        logvol = -math.log(2) * (1. + np.arange(niter))
+        if added_live:
+            logvol = np.append(logvol, (logvol[-1] if niter else 0.0) + math.log(0.5))
+        logwt, logz, logzvar, h = _integrate(logl, logvol)
+        nc = np.asarray(res['ncall_per_it'])[sel]
+        r = Results(nlive=1, niter=niter, ncall_per_it=nc, eff=100. * nsamps / max(int(nc.sum()), 1), logl=logl,
+                    logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(logzvar), information=h)
+        for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch'):
+            if k in res and len(res[k]) == len(ids):
+                r[k] = np.asarray(res[k])[sel]
+        if 'batch_bounds' in res:
+            r['batch_bounds'] = res['batch_bounds']
+        out.append(r)
+    return out

@@ -317,6 +317,36 @@ int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, 
                     uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
                     double* logvol_full, double* logwt_full, double* logz_full, double* kld_full);
 
+/* ---- run uncertainties: resample_run (utils.py:1495-1660 of the reference) ----------------------------------------
+ * R bootstrap realisations of one record of N samples (logl ascending) made of S strands (strand[i] in 0..S-1, the
+ * compacted samples_id).  Strand s is a BASE strand when base[s] != 0 (one of its samples belongs to a batch whose
+ * lower bound is -inf), else an add-on strand.  Realisation r draws from the B2N stream (seed, chain0 + r) in the
+ * reference's call order, so the unmodified reference driven by oracle.resample.ScriptedResampleGenerator(seed,
+ * chain0 + r) consumes the same numbers:
+ *   tick 0   one uniform vector event of nbase elements; element e picks base strand
+ *            base_ids[min(floor(U_e * nbase), nbase - 1)], base_ids = the base strands in increasing order
+ *   tick 1   the same over the nadd add-on strands, present only when nadd > 0.
+ * m[s] = the times strand s is drawn.  Sample i appears m[strand[i]] times in the realisation.
+ * Live counts (the strand rule): sample p is one PIECE of its strand, live on (birth_p, logl_p]; birth_p is the
+ * threshold p entered the live set above.  The piece plan is built on the host: piece_ptr (N + 1) and piece_strand
+ * form a CSR of the pieces whose first covered sample is i (a piece covers samples first..p); pieces of live points
+ * that were never recorded (a record without its final live points) are listed with their strand and never end.
+ * The count at sample i is n_i = sum over the pieces covering it of m of their strand.  Its m copies get ln X
+ * increments ln(n/(n+1)) each, except at a strand's last sample when end[i] != 0 (a final live point): there the
+ * copies get n, n-1, .., n-m+1 live points, a total increment of ln((n-m+1)/(n+1)).
+ * Then the trapezoid integrals of compute_integrals (:1411-1467) over the copies give logz, logzvar and h, and
+ * kld = sum of p1 (ln p1 - ln p2), ln p1 = logwt - logz[-1], ln p2 = logwt_ref - logz_ref of the copy's sample
+ * (kld_error, :1976-1992).  logwt_ref NULL: no KL divergence (kld must then be NULL).
+ * FP64; one CTA per realisation scans the record, so realisation r does not depend on R (R <= 65535).
+ * strand, base, piece_ptr, piece_strand, end: HOST.  logl, logwt_ref: N.  end may be NULL (no strand ends).
+ * Summary outputs, R each, each may be NULL: logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1], kld[-1].
+ * mult: R x S row-major int32 (m of every strand), may be NULL.  Two kernel launches whatever R, N or S.
+ * Synchronises in host-pointer mode. */
+int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                      const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
+                      const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
+                      double* logz, double* logzerr, double* h, double* kld, int32_t* mult);
+
 /* ---- resident bound for the proposal kernels --------------------------------
  * Uploads K ellipsoids of dimension ncdim (what Sampler ships to every task as
  * `axes` / kwargs['bound'], sampler.py:708-717, internal_samplers.py:229-233).
@@ -543,6 +573,16 @@ int b2n_ns_reserve_dead(b2n_ctx* ctx, int64_t capacity);
 int b2n_ns_get_live(b2n_ctx* ctx, double* live_u, double* live_v, double* live_logl);
 int b2n_ns_get_dead(b2n_ctx* ctx, int64_t first, int64_t count, double* u, double* v, double* logl,
                     double* logvol, int32_t* ncall);
+/* Strands (the reference's samples_id / samples_it, sampler.py:1107, 1182).  Every round records, for its j-th removal,
+ * the live slot it occupied (slot[it0 + j] = its row in the live set) and the number of dead rows recorded before it
+ * entered the live set (it[it0 + j]); the slot's new occupant then gets it0 + K, the dead rows after the round, so its
+ * birth threshold is the logl of dead row it0 + K - 1, the round threshold.  Unit-cube rounds record the same.  Counts
+ * are in the numbering of this device buffer (row 0 = the first row after b2n_ns_set_state); b2n_ns_set_state sets
+ * every slot's count to 0, b2n_ns_set_live_it replaces them (a hand-over from a host loop or a checkpoint, in the
+ * same numbering: negative for points that entered before row 0).  Host outputs (each may be NULL), N = nlive. */
+int b2n_ns_get_strands(b2n_ctx* ctx, int64_t first, int64_t count, int32_t* slot, int64_t* it);
+int b2n_ns_set_live_it(b2n_ctx* ctx, const int64_t* live_it);
+int b2n_ns_get_live_it(b2n_ctx* ctx, int64_t* live_it);
 
 #ifdef __cplusplus
 }
