@@ -238,8 +238,8 @@ __device__ __forceinline__ void ball_direction_pair_fast(const ChainRng& ga, con
 
 // One direction with the branch-free math, WITHOUT the step factor: z -> b2n_sm[off..] (when `store`), returns the
 // warp-reduced |z|^2 and log(U) of the radius uniform (lane 31's block, see ball_direction).  The caller forms
-// U^(1/nc) / |z| later -- rwalk_mma16_kernel does that for a whole ring of items at once, one LANE per item,
-// instead of once per item on all 32 lanes.  Same draw events, ticks and arithmetic as ball_direction_pair_fast.
+// U^(1/nc) / |z| later -- the draw warps of rwalk_mmaws_kernel do that for a whole ring of items at once, one LANE
+// per item, instead of once per item on all 32 lanes.  Same draw events, ticks and arithmetic as ball_direction_pair_fast.
 __device__ __forceinline__ void ball_draw_fast(const ChainRng& g, int off, bool store, int nc, int lane, double& ss,
                                                double& lgU) {
     const int nb = (nc + 1) >> 1;

@@ -1,6 +1,6 @@
-// b2n_rwalk.cu -- batched random-walk proposal chains: a warp-per-chain kernel (this comment), and two
-// lock-step FP64-tensor-core kernels further down (rwalk_mma_kernel: the default for 16 <= n <= 64,
-// rwalk_mmas_kernel: n > 64).
+// b2n_rwalk.cu -- batched random-walk proposal chains: a warp-per-chain kernel (this comment), and three
+// lock-step FP64-tensor-core kernels further down (rwalk_mma_kernel and its warp-specialised form
+// rwalk_mmaws_kernel for 16 <= n <= 64, rwalk_mmas_kernel for n > 64).  rwalk_plan picks one per call.
 //
 // Replaces RWalkSampler.sample -> generic_random_walk -> propose_ball_point
 // (reference internal_samplers.py:505-561, 866-986, 989-1035) for a whole queue
@@ -53,6 +53,7 @@ __device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double
                  : "d"(a), "d"(b));
 }
 
+// Shared-memory plan of rwalk_mma_kernel, in doubles: the kernel takes its offsets from it, the host its size.
 // KT = k-tiles of 4 columns (n <= 4*KT); CH = chains in lock-step per CTA (8 -> 256 threads, two
 // CTAs per SM overlap each other's barriers instead of one 16-chain CTA per SM waiting at each).
 // DEPTH = direction ring: the draws of a step do not depend on the chain state (the Philox counter
@@ -61,15 +62,32 @@ __device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double
 // (8 chains) gains a barrier per step; a CTA with few chains -- the small rounds of b2n_ns_run run
 // one chain per CTA -- generates its directions on 8 warps in parallel instead of serially on one,
 // which is the longest dependency chain of a step (Philox -> log -> sqrt -> sincospi).
-// FAST = the draws use the branch-free math of b2n_fastmath.cuh, two ring items at a time per warp
-// (the default; B2N_RWALK_DRAWS=libm selects libdevice math, results differ by a few ulp in the directions).
-template <int LIKE, int KT, int CH, int DEPTH, bool FAST>
-__global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(const RwalkParams p) {
-    constexpr int B2N_MMA_CH = CH;
-    constexpr int RS = 8 * ((4 * KT + 7) / 8);                    // rows padded to whole 8-row slabs
-    constexpr int XS = RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16));   // chain stride == 4 (mod 16):
-                                                                  // the B-fragment loads are conflict free
-    constexpr int YS = RS + 2;
+template <int KT>
+struct MmaLayout {
+    static constexpr int CH = 8, DEPTH = 8;
+    static constexpr int RS = 8 * ((4 * KT + 7) / 8);                    // rows padded to whole 8-row slabs
+    static constexpr int XS = RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16));   // chain stride == 4 (mod 16):
+                                                                         // the B-fragment loads are conflict free
+    static constexpr int YS = RS + 2;
+    static constexpr int XB = CH * XS;                                   // one direction buffer (all chains of the CTA)
+    int n, npad;
+    __host__ __device__ explicit MmaLayout(int n_) : n(n_), npad((n_ + 1) & ~1) {}
+    __host__ __device__ int o_fl() const { return 4 * npad; }           // dimension flags, after stage_model's vectors
+    // ring: direction z of step s, later delta = v - mean
+    __host__ __device__ int o_x() const { return o_fl() + (((n + 3) >> 2) << 1); }
+    __host__ __device__ int o_y() const { return o_x() + DEPTH * XB; }  // axes @ z (chain-major)
+    __host__ __device__ int o_q() const { return o_y() + CH * YS; }     // per-slab partial quadratic forms
+    __host__ __device__ int o_f() const { return o_q() + 8 * CH; }      // step factors scale * U^(1/n) / |z|
+    __host__ __device__ int o_st() const { return o_f() + DEPTH * CH; } // per-chain state: ucur, uprop, vcur, vprop
+    __host__ __device__ int total() const { return o_st() + CH * 4 * npad; }
+};
+
+// The draws use the branch-free math of b2n_fastmath.cuh, two ring items at a time per warp, where lane 31 is idle
+// (n <= 62); at n = 63, 64 one item at a time with ball_direction.
+template <int LIKE, int KT>
+__global__ void __launch_bounds__(256, 2) rwalk_mma_kernel(const RwalkParams p) {
+    using L = MmaLayout<KT>;
+    constexpr int CH = L::CH, DEPTH = L::DEPTH, XS = L::XS, YS = L::YS, XB = L::XB;
     const int n = p.n;
     const int npad = (n + 1) & ~1;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -77,19 +95,12 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
     const int3 cd = p.cta[blockIdx.x];
     const int S = (n + 7) >> 3;                     // 8-row slabs
     // ---- shared-memory plan
-    int off = 0;
-    const ModelSm ms = stage_model(p.m, off, n, npad);
+    const L lay(n);
+    const ModelSm ms = stage_model(p.m, 0, n, npad);
     const int op0 = ms.op0, op1 = ms.op1, omu = ms.olv0;
-    off += 4 * npad;
-    uint32_t* fl = reinterpret_cast<uint32_t*>(&b2n_sm[off]);
+    uint32_t* fl = reinterpret_cast<uint32_t*>(&b2n_sm[lay.o_fl()]);
     for (int i = threadIdx.x; i < n; i += blockDim.x) fl[i] = p.dimflags ? p.dimflags[i] : 0u;
-    off += ((n + 3) >> 2) << 1;
-    constexpr int XB = B2N_MMA_CH * XS;             // one direction buffer (all chains of the CTA)
-    const int oX = off;  off += DEPTH * XB;         // ring: direction z of step s, later delta = v - mean
-    const int oY = off;  off += B2N_MMA_CH * YS;    // axes @ z (chain-major)
-    const int oQ = off;  off += 8 * B2N_MMA_CH;     // per-slab partial quadratic forms
-    const int oF = off;  off += DEPTH * B2N_MMA_CH; // step factors scale * U^(1/n) / |z|
-    const int ost = off;                            // per-chain state: ucur, uprop, vcur, vprop
+    const int oX = lay.o_x(), oY = lay.o_y(), oQ = lay.o_q(), oF = lay.o_f(), ost = lay.o_st();
     for (int e = threadIdx.x; e < DEPTH * XB; e += blockDim.x) b2n_sm[oX + e] = 0.0;
     // ---- matrix fragments -> registers.  item (s, t): slab s of rows, chain tile t
     const int s_it = warp % S, t_it = warp / S;
@@ -111,9 +122,9 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
     const double inv_n = 1.0 / (double)n;
     const int pk = p.m.prior_kind;
 
-    for (int g0 = 0; g0 < cd.y; g0 += B2N_MMA_CH) {             // groups of CH chains
+    for (int g0 = 0; g0 < cd.y; g0 += CH) {                     // groups of CH chains
         const int c = warp;                                     // chain slot owned by this warp
-        const int nlc = (cd.y - g0) < B2N_MMA_CH ? (cd.y - g0) : B2N_MMA_CH;   // live chains of the group
+        const int nlc = (cd.y - g0) < CH ? (cd.y - g0) : CH;    // live chains of the group
         const bool live = c < nlc;
         const int q = live ? p.order[cd.x + g0 + c] : 0;
         int oucur = ost + c * 4 * npad, ouprop = oucur + npad, ovcur = ouprop + npad, ovprop = ovcur + npad;
@@ -126,9 +137,9 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
             // ---- phase 1 (all warps): directions in the unit ball of the next DEPTH steps of every
             //      live chain -> X[s][chain], factors -> F[s][chain].  Item w = (step s, chain c2).
             const int nd = (p.walks - step0) < DEPTH ? (p.walks - step0) : DEPTH;
-            if (FAST && n <= 62) {
-                for (int w = warp; w < nd * nlc; w += 2 * B2N_MMA_CH) {       // items w and w + CH together
-                    const int w2 = w + B2N_MMA_CH;
+            if (n <= 62) {
+                for (int w = warp; w < nd * nlc; w += 2 * CH) {         // items w and w + CH together
+                    const int w2 = w + CH;
                     const bool two = w2 < nd * nlc;
                     const int sa = w / nlc, ca = w - sa * nlc;
                     const int sb = two ? w2 / nlc : sa, cb = two ? w2 - sb * nlc : ca;
@@ -141,23 +152,23 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
                     ball_direction_pair_fast(ga, gb, oX + sa * XB + ca * XS, oX + sb * XB + cb * XS, two, n, lane, inv_n,
                                              fa, fb);
                     if (lane == 0) {
-                        b2n_sm[oF + sa * B2N_MMA_CH + ca] = scale_ * fa;
-                        if (two) b2n_sm[oF + sb * B2N_MMA_CH + cb] = scale_ * fb;
+                        b2n_sm[oF + sa * CH + ca] = scale_ * fa;
+                        if (two) b2n_sm[oF + sb * CH + cb] = scale_ * fb;
                     }
                 }
             } else
-            for (int w = warp; w < nd * nlc; w += B2N_MMA_CH) {
+            for (int w = warp; w < nd * nlc; w += CH) {
                 const int s = w / nlc, c2 = w - s * nlc;
                 ChainRng g;
                 g.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + c2]);
                 g.tick = 2u * (uint32_t)(step0 + s);             // two draw events per step (:1011-1016)
                 const double f = scale_ * ball_direction(g, oX + s * XB + c2 * XS, n, lane, inv_n);
-                if (lane == 0) b2n_sm[oF + s * B2N_MMA_CH + c2] = f;
+                if (lane == 0) b2n_sm[oF + s * CH + c2] = f;
             }
             __syncthreads();
             for (int s = 0; s < nd; s++) {
             const int oXs = oX + s * XB, ox = oXs + c * XS;
-            const double fac = live ? b2n_sm[oF + s * B2N_MMA_CH + c] : 0.0;
+            const double fac = live ? b2n_sm[oF + s * CH + c] : 0.0;
             // ---- phase 2 (item warp): Y[rows of slab][chains of tile] = A_slab @ X
             if (has_item) {
                 // NACC independent accumulator pairs: the k-tiles form NACC short DMMA dependency chains instead
@@ -216,14 +227,14 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
                         q1 += __shfl_xor_sync(B2N_FULL, q1, o);
                     }
                     if (lane < 4) {
-                        b2n_sm[oQ + s_it * B2N_MMA_CH + c0] = q0;
-                        b2n_sm[oQ + s_it * B2N_MMA_CH + c0 + 1] = q1;
+                        b2n_sm[oQ + s_it * CH + c0] = q0;
+                        b2n_sm[oQ + s_it * CH + c0 + 1] = q1;
                     }
                 }
                 __syncthreads();
                 // ---- phase 5 (chain warp): logl
                 double qf = 0.0;
-                for (int s2 = 0; s2 < S; s2++) qf += b2n_sm[oQ + s2 * B2N_MMA_CH + c];
+                for (int s2 = 0; s2 < S; s2++) qf += b2n_sm[oQ + s2 * CH + c];
                 l = fma(-0.5, qf, p.m.s0);
             } else {
                 if (live && ok) {
@@ -275,264 +286,6 @@ __global__ void __launch_bounds__(CH * 32, CH == 8 ? 2 : 1) rwalk_mma_kernel(con
 }
 
 // =====================================================================================
-// rwalk_mma16_kernel -- the lock-step kernel above re-cut for SIXTEEN warps per 8 chains (GAUSS_PREC models).
-//
-// Why: rwalk_mma_kernel is bound by dependent-instruction latency -- 2 CTAs x 8 warps per SM
-// (128 registers) leave most issue cycles idle -- and a 2000-chain queue has only ~15 chains per SM, so more CTAs cannot be made resident.  The same work is therefore dealt over twice the warps,
-// and the instruction count per step is cut:
-//   * contractions: item = (8-row slab, HALF of the k-tiles) -> 2 S <= 16 item warps with 7 instead of 13 dependent
-//     DMMAs, and 7 + 7 instead of 13 + 13 fragment registers per thread (<= 64 registers: 2 CTAs x 512 threads);
-//     the two partial sums meet in shared memory (phase 3 adds the halves of y, phase 5 the 2 S partial forms);
-//   * chain phases: two warps per chain, lane = component, so a thread owns ONE component of its chain for the whole
-//     kernel: the chain state (u, v, and the proposal) lives in registers, not in shared memory;
-//   * every shared-memory offset is a compile-time constant (the layout depends on KT only, not on n);
-//   * two CTA barriers per step instead of three: the item warps run phase 4 of step s and phase 2 of step s + 1
-//     back to back, the chain warps phase 5 of step s and phase 3 of step s + 1 (phase 2 does not depend on the
-//     accept / reject of the step before: the directions are in the ring);
-//   * draws: the ring items are dealt over 16 warps, and the step factor scale * U^(1/n) / |z| (exp, divide, sqrt) is
-//     no longer computed on all 32 lanes per item but for the whole ring at once with one LANE per item, by the two
-//     warps that have no contraction item (the first two when S = 8) while the others run phase 2 of the first step.
-// Draw events, ticks and the arithmetic of every draw are those of rwalk_mma_kernel; only the summation order of the
-// two contractions differs (round-off).
-// =====================================================================================
-template <int KT>
-struct Mma16Layout {
-    static constexpr int CH = 8, NW = 16, DEPTH = 8;
-    static constexpr int KH = (KT + 1) / 2;                              // k-tiles per half
-    static constexpr int RS = 8 * ((4 * KT + 7) / 8);                    // rows padded to whole slabs (>= n)
-    static constexpr int XS = RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16));
-    static constexpr int YS = RS + 2;
-    static constexpr int XB = CH * XS;
-    static constexpr int O_P0 = 0, O_P1 = RS;                            // prior vectors (mean, flags: registers)
-    static constexpr int O_X = 2 * RS;                                   // ring: direction z of step s, later delta = v - mean
-    static constexpr int O_Y = O_X + DEPTH * XB;                         // the two k-halves of axes @ z (chain-major)
-    static constexpr int O_Q = O_Y + 2 * CH * YS;                        // partial quadratic forms per (slab, half)
-    static constexpr int O_F = O_Q + 16 * CH;                            // step factors per ring slot
-    static constexpr int O_SS = O_F + DEPTH * CH;                        // |z|^2 per ring slot
-    static constexpr int O_LG = O_SS + DEPTH * CH;                       // log U of the radius per ring slot
-    static constexpr int O_OK = O_LG + DEPTH * CH;                       // in-cube flags [step parity][chain][half]
-    static constexpr int TOTAL = O_OK + 16;                              // doubles
-};
-
-template <int KT>
-__global__ void __launch_bounds__(512, 2) rwalk_mma16_kernel(const RwalkParams p) {
-    using L = Mma16Layout<KT>;
-    constexpr int CH = L::CH, NW = L::NW, DEPTH = L::DEPTH, KH = L::KH, XS = L::XS, YS = L::YS, XB = L::XB;
-    const int n = p.n;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    B2N_DYN_PROLOGUE(p)
-    const int3 cd = p.cta[blockIdx.x];
-    const int S = (n + 7) >> 3;
-    int* okf = reinterpret_cast<int*>(&b2n_sm[L::O_OK]);
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        b2n_sm[L::O_P0 + i] = p.m.pp0 ? p.m.pp0[i] : 0.0;
-        b2n_sm[L::O_P1 + i] = p.m.pp1 ? p.m.pp1[i] : 1.0;
-    }
-    for (int e = threadIdx.x; e < DEPTH * XB; e += blockDim.x) b2n_sm[L::O_X + e] = 0.0;
-    // ---- fragments: item (slab s_it, half h_it) of both matrices
-    const int s_it = warp % S, h_it = warp / S;
-    const bool has_item = warp < 2 * S;
-    double fragA[KH], fragP[KH];
-    {
-        const double* Ag = p.axesT + (size_t)cd.z * n * n;
-        const double* Pg = p.m.lmat;
-        const int row = 8 * s_it + (lane >> 2);
-#pragma unroll
-        for (int j = 0; j < KH; j++) {
-            const int col = 4 * (h_it * KH + j) + (lane & 3);
-            const bool in = has_item && row < n && col < n;
-            fragA[j] = in ? Ag[(size_t)col * n + row] : 0.0;
-            fragP[j] = in ? Pg[(size_t)row * n + col] : 0.0;
-        }
-    }
-    // item-phase addresses (relative to the ring slot of the step)
-    const int xb_it = (lane >> 2) * XS + (lane & 3) + 4 * h_it * KH;           // B fragment of k-tile 0 of the half
-    const int yst_it = L::O_Y + (h_it * CH + 2 * (lane & 3)) * YS + 8 * s_it + (lane >> 2);
-    const int xr_it = 2 * (lane & 3) * XS + 8 * s_it + (lane >> 2);            // delta[row] of chain c0
-    // the two warps that turn (|z|^2, log U) of the ring into step factors: those without an item, else the first two
-    const int fw = (2 * S <= NW - 2) ? warp - (NW - 2) : warp;
-    const double inv_n = 1.0 / (double)n;
-    const int pk = p.m.prior_kind;
-    const int c = warp >> 1, hh = warp & 1;                       // chain slot and component half of this warp
-    const int ci = 32 * hh + lane;                                // the component this thread owns
-    const bool cin = ci < n;
-    const uint32_t myfl = cin ? (p.dimflags ? p.dimflags[ci] : 0u) : 0u;
-    const double mymu = cin && p.m.lv0 ? p.m.lv0[ci] : 0.0;
-    __syncthreads();
-
-    for (int g0 = 0; g0 < cd.y; g0 += CH) {
-        const int nlc = (cd.y - g0) < CH ? (cd.y - g0) : CH;
-        const bool live = c < nlc;
-        const int q = live ? p.order[cd.x + g0 + c] : 0;
-        double ucur = (live && cin) ? p.u0[(size_t)(p.start ? p.start[q] : q) * n + ci] : 0.0, vcur = 0.0, uprop = 0.0, vprop = 0.0;
-        int nacc = 0, nrej = 0;
-        double lcur = 0.0;
-
-        // phase 2 of ring slot s: Y_h[rows of slab][chains] = A_slab[:, half h] @ X[half h]
-        auto phase2 = [&](int oXs) {
-            double d0 = 0.0, d1 = 0.0, e0 = 0.0, e1 = 0.0;
-            const int xb = oXs + xb_it;
-#pragma unroll
-            for (int j = 0; j + 1 < KH; j += 2) {
-                dmma884(d0, d1, fragA[j], b2n_sm[xb + 4 * j]);
-                dmma884(e0, e1, fragA[j + 1], b2n_sm[xb + 4 * j + 4]);
-            }
-            if (KH & 1) dmma884(d0, d1, fragA[KH - 1], b2n_sm[xb + 4 * (KH - 1)]);
-            b2n_sm[yst_it] = d0 + e0;
-            b2n_sm[yst_it + YS] = d1 + e1;
-        };
-        // phase 3 of ring slot s: u' = u + fac*y, wrap / reflect / cube test, prior, delta -> X[s][c]
-        auto phase3 = [&](int s) {
-            bool ok = true;
-            if (cin) {
-                const double fac = b2n_sm[L::O_F + s * CH + c];
-                const double y = b2n_sm[L::O_Y + c * YS + ci] + b2n_sm[L::O_Y + (CH + c) * YS + ci];
-                double t = fma(fac, y, ucur);
-                if (myfl & B2N_DIM_PERIODIC) t = mod1(t);
-                if (myfl & B2N_DIM_REFLECTIVE) t = reflect1(t);
-                ok = in_cube(t, myfl);
-                uprop = t;
-                vprop = prior_sm(pk, L::O_P0, L::O_P1, ci, t);
-                b2n_sm[L::O_X + s * XB + c * XS + ci] = vprop - mymu;
-            }
-            ok = __all_sync(B2N_FULL, ok);
-            if (lane == 0) okf[(s & 1) * 16 + warp] = ok ? 1 : 0;
-        };
-        // phase 4 of ring slot s: partial delta^T P delta over (rows of the slab) x (columns of the half)
-        auto phase4 = [&](int oXs) {
-            double d0 = 0.0, d1 = 0.0, e0 = 0.0, e1 = 0.0;
-            const int xb = oXs + xb_it;
-#pragma unroll
-            for (int j = 0; j + 1 < KH; j += 2) {
-                dmma884(d0, d1, fragP[j], b2n_sm[xb + 4 * j]);
-                dmma884(e0, e1, fragP[j + 1], b2n_sm[xb + 4 * j + 4]);
-            }
-            if (KH & 1) dmma884(d0, d1, fragP[KH - 1], b2n_sm[xb + 4 * (KH - 1)]);
-            double q0 = (d0 + e0) * b2n_sm[oXs + xr_it], q1 = (d1 + e1) * b2n_sm[oXs + xr_it + XS];
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-                q0 += __shfl_xor_sync(B2N_FULL, q0, o);
-                q1 += __shfl_xor_sync(B2N_FULL, q1, o);
-            }
-            if (lane < 4) {
-                b2n_sm[L::O_Q + warp * CH + 2 * lane] = q0;
-                b2n_sm[L::O_Q + warp * CH + 2 * lane + 1] = q1;
-            }
-        };
-        // phase 5 of ring slot s (both warps of the chain, identically): logl, accept / reject
-        auto phase5 = [&](int s) {
-            double qf = (lane < 2 * S) ? b2n_sm[L::O_Q + lane * CH + c] : 0.0;     // 2 S <= 16 partials
-#pragma unroll
-            for (int o = 8; o > 0; o >>= 1) qf += __shfl_xor_sync(B2N_FULL, qf, o);
-            qf = __shfl_sync(B2N_FULL, qf, 0);
-            const double l = fma(-0.5, qf, p.m.s0);
-            const int* ok2 = &okf[(s & 1) * 16 + 2 * c];
-            const bool ok = (ok2[0] & ok2[1]) != 0;
-            if (ok && l > loglstar_) {
-                ucur = uprop;
-                vcur = vprop;
-                lcur = l;
-                nacc++;
-            } else {
-                nrej++;
-            }
-        };
-
-        for (int step0 = 0; step0 < p.walks; step0 += DEPTH) {
-            const int nd = (p.walks - step0) < DEPTH ? (p.walks - step0) : DEPTH;
-            const int nit = nd * nlc;
-            // ---- phase 1 (all warps): the directions of the next nd steps of every live chain
-            if (nit > NW) {
-                for (int w = warp; w < nit; w += 2 * NW) {        // two items side by side (their chains interleave)
-                    const int w2 = w + NW;
-                    const bool two = w2 < nit;
-                    int sa, ca, sb, cb;
-                    if (nlc == CH) { sa = w >> 3; ca = w & 7; sb = w2 >> 3; cb = w2 & 7; }
-                    else { sa = w / nlc; ca = w - sa * nlc; sb = w2 / nlc; cb = w2 - sb * nlc; }
-                    if (!two) { sb = sa; cb = ca; }
-                    ChainRng ga, gb;
-                    ga.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + ca]);
-                    gb.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + cb]);
-                    ga.tick = 2u * (uint32_t)(step0 + sa);
-                    gb.tick = 2u * (uint32_t)(step0 + sb);
-                    double ssa, lga, ssb, lgb;
-                    ball_draw_fast(ga, L::O_X + sa * XB + ca * XS, true, n, lane, ssa, lga);
-                    ball_draw_fast(gb, L::O_X + sb * XB + cb * XS, two, n, lane, ssb, lgb);
-                    if (lane == 0) {
-                        b2n_sm[L::O_SS + sa * CH + ca] = ssa;
-                        b2n_sm[L::O_LG + sa * CH + ca] = lga;
-                        if (two) {
-                            b2n_sm[L::O_SS + sb * CH + cb] = ssb;
-                            b2n_sm[L::O_LG + sb * CH + cb] = lgb;
-                        }
-                    }
-                }
-            } else if (warp < nit) {                              // few chains (b2n_ns_run's rounds): one item per warp
-                const int sa = warp / nlc, ca = warp - sa * nlc;
-                ChainRng ga;
-                ga.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + ca]);
-                ga.tick = 2u * (uint32_t)(step0 + sa);
-                double ssa, lga;
-                ball_draw_fast(ga, L::O_X + sa * XB + ca * XS, true, n, lane, ssa, lga);
-                if (lane == 0) {
-                    b2n_sm[L::O_SS + sa * CH + ca] = ssa;
-                    b2n_sm[L::O_LG + sa * CH + ca] = lga;
-                }
-            }
-            __syncthreads();
-            // ---- step factors of the whole ring, one lane per ring slot (step e / CH, chain e % CH)
-            if (fw == 0 || fw == 1) {
-                const int e = 32 * fw + lane;
-                if (e < nd * CH && (e & (CH - 1)) < nlc)
-                    b2n_sm[L::O_F + e] = scale_ * b2n_div(exp(b2n_sm[L::O_LG + e] * inv_n), b2n_sqrt(b2n_sm[L::O_SS + e]));
-            }
-            if (has_item) phase2(L::O_X);
-            __syncthreads();
-            if (live) phase3(0);
-            __syncthreads();
-            for (int s = 0; s < nd; s++) {
-                if (has_item) {
-                    phase4(L::O_X + s * XB);
-                    if (s + 1 < nd) phase2(L::O_X + (s + 1) * XB);
-                }
-                __syncthreads();
-                if (live) phase5(s);
-                if (s + 1 < nd) {
-                    if (live) phase3(s + 1);
-                    __syncthreads();
-                }
-            }
-            // (the next ring is drawn in the same barrier interval as phase 5 of the last step: every read of the ring
-            //  -- phase 4 of that step -- sits before the barrier above)
-        }
-        // no accept: (v, logl) of the start point are recomputed (:970-975); every thread its own component of v
-        if (live && nacc == 0 && cin) {
-            vcur = prior_sm(pk, L::O_P0, L::O_P1, ci, ucur);
-            b2n_sm[L::O_Y + c * YS + ci] = vcur - mymu;
-        }
-        __syncthreads();
-        if (live) {
-            if (nacc == 0 && hh == 0)
-                lcur = fma(-0.5, quadform_full<false>(p.m.lmat, 0, n, n, L::O_Y + c * YS, lane), p.m.s0);
-            if (cin) {
-                peer_put(p.peer, &p.u[(size_t)q * n + ci], ucur);
-                peer_put(p.peer, &p.v[(size_t)q * n + ci], vcur);
-            }
-            if (lane == 0 && hh == 0) {
-                peer_put(p.peer, &p.logl[q], lcur);
-                peer_put(p.peer, &p.nacc[q], nacc);
-                peer_put(p.peer, &p.nrej[q], nrej);
-                peer_put(p.peer, &p.ncall[q], (int)p.walks);
-            }
-        }
-        __syncthreads();
-        for (int e = threadIdx.x; e < DEPTH * XB; e += blockDim.x) b2n_sm[L::O_X + e] = 0.0;
-        __syncthreads();
-    }
-    peer_finish(p.peer);
-}
-
-// =====================================================================================
 // rwalk_mmaws_kernel -- the lock-step kernel, WARP-SPECIALISED (GAUSS_PREC models): 8 step warps + 4 draw warps.
 //
 // Why: the draws are a large share of the instructions of rwalk_mma_kernel and the only part of it that is
@@ -547,9 +300,10 @@ __global__ void __launch_bounds__(512, 2) rwalk_mma16_kernel(const RwalkParams p
 //     step s + 1 run back to back, then phase 5 of step s and phase 3 of step s + 1);
 //   * the two roles meet at named barriers only (FULL / EMPTY per ring buffer: bar.arrive on one side, bar.sync on
 //     the other), the step warps synchronise among themselves on a 256-thread named barrier;
-//   * setmaxnreg moves registers from the draw warps to the step warps (the fragments alone are 52 registers).
-// Draw events, ticks and arithmetic are those of rwalk_mma_kernel (the step factor is the same expression); the
-// contractions are summed in the same order: results are bit-identical to rwalk_mma_kernel with fast draws.
+//   * setmaxnreg moves registers from the draw warps (64) to the step warps (88; the fragments alone are 52 registers):
+//     256 x 88 + 128 x 64 = the 384 x 80 the CTA is launched with.
+// Draw events, ticks and arithmetic are those of rwalk_mma_kernel (the step factor is the same expression); delta^T P
+// delta is summed as 2 delta^T U delta (below), so results agree with rwalk_mma_kernel to round-off.
 // =====================================================================================
 template <int KT>
 struct MmaWsLayout {
@@ -642,14 +396,12 @@ __device__ __forceinline__ void nbar_arrive(int id, int count) {
     asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// SETREG: 0 = every warp keeps the 80 registers of the launch; 1 = 88 (step) / 64 (draw); 2 = 96 / 48
-// (256 x step + 128 x draw must not exceed the 384 x 80 registers the CTA is launched with; only 1 is instantiated).
 // PLAIN: no periodic / reflective dimension and a prior that is affine per component (uniform, identity): phase 3 is
 // then straight-line code for the (at most) two components of a lane.
 // Ring: RB = 2 buffers of DB = 8 steps; the step warps start every buffer with a two-interval prologue.  Not kept: ONE
 // pipeline over all ring slots, the next buffer awaited where it is first touched (two steps early) -- the draw warps are
 // busy most of the time, and taking two steps of slack away from them makes both roles wait for each other.
-template <int KT, int SETREG, bool PLAIN>
+template <int KT, bool PLAIN>
 __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p) {
     using L = MmaWsLayout<KT>;
     constexpr int CH = L::CH, XS = L::XS, YS = L::YS, XB = L::XB, RS = L::RS;
@@ -672,8 +424,7 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
 
     if (warp >= L::NSW) {
         // =============================== draw warps ===============================
-        if (SETREG == 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-        if (SETREG == 2) asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
         const int dw = warp - L::NSW;
         const double inv_n = 1.0 / (double)n;
         for (int g0 = 0; g0 < cd.y; g0 += CH) {
@@ -731,8 +482,7 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
         }
     } else {
         // =============================== step warps ===============================
-        if (SETREG == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 88;");
-        if (SETREG == 2) asm volatile("setmaxnreg.inc.sync.aligned.u32 96;");
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 88;");
         const int S = (n + 7) >> 3;
         const int s_it = warp;                                    // slab of this warp's item of axes @ z
         const bool has_item = warp < S;
@@ -942,26 +692,41 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
 // n^2*8/16 bytes instead of the n^2*8 of the warp-per-chain kernel (20 KB vs 320 KB at n=200).
 // Warp w owns slabs w, w+16, ...  BASELINE config C4 (200-D, single ellipsoid, rwalk).
 // =====================================================================================
+// Shared-memory plan of rwalk_mmas_kernel, in doubles: the kernel takes its offsets from it, the host its size.
+struct MmasLayout {
+    static constexpr int CH = 16;
+    int n, npad;
+    int RS, XS, YS; // rows padded to whole 8-row slabs; chain strides of X (== 4 mod 16: conflict-free B fragments), Y
+    __host__ __device__ explicit MmasLayout(int n_)
+        : n(n_), npad((n_ + 1) & ~1), RS(8 * ((n_ + 7) / 8)), XS(RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16))),
+          YS(RS + 2) {}
+    __host__ __device__ int o_fl() const { return 4 * npad; }           // dimension flags, after stage_model's vectors
+    // direction z, later delta = v - mean (chain-major)
+    __host__ __device__ int o_x() const { return o_fl() + (((n + 3) >> 2) << 1); }
+    __host__ __device__ int o_y() const { return o_x() + CH * XS; }     // axes @ z (chain-major)
+    __host__ __device__ int o_q() const { return o_y() + CH * YS; }     // per-slab partial quadratic forms
+    __host__ __device__ int o_st() const { return o_q() + (RS / 8) * CH; }  // per-chain state: ucur, uprop, vcur, vprop
+    // helper scratch: step factors, U^(1/n), current state buffers, cube flags (CH x CH ints)
+    __host__ __device__ int o_h() const { return o_st() + CH * 4 * npad; }
+    __host__ __device__ int total() const { return o_h() + 3 * CH + CH * CH / 2; }
+};
+
 template <int LIKE>
-__global__ void __launch_bounds__(512, 1) rwalk_mmas_kernel(const RwalkParams p, int XS, int YS) {
-    constexpr int CH = 16;
+__global__ void __launch_bounds__(512, 1) rwalk_mmas_kernel(const RwalkParams p) {
+    constexpr int CH = MmasLayout::CH;
     const int n = p.n;
     const int npad = (n + 1) & ~1;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     B2N_DYN_PROLOGUE(p)
     const int3 cd = p.cta[blockIdx.x];
     const int S = (n + 7) >> 3, KT = (n + 3) >> 2;
-    int off = 0;
-    const ModelSm ms = stage_model(p.m, off, n, npad);
+    const MmasLayout lay(n);
+    const int XS = lay.XS, YS = lay.YS;
+    const ModelSm ms = stage_model(p.m, 0, n, npad);
     const int op0 = ms.op0, op1 = ms.op1, omu = ms.olv0;
-    off += 4 * npad;
-    uint32_t* fl = reinterpret_cast<uint32_t*>(&b2n_sm[off]);
+    uint32_t* fl = reinterpret_cast<uint32_t*>(&b2n_sm[lay.o_fl()]);
     for (int i = threadIdx.x; i < n; i += blockDim.x) fl[i] = p.dimflags ? p.dimflags[i] : 0u;
-    off += ((n + 3) >> 2) << 1;
-    const int oX = off;  off += CH * XS;
-    const int oY = off;  off += CH * YS;
-    const int oQ = off;  off += S * CH;
-    const int ost = off;
+    const int oX = lay.o_x(), oY = lay.o_y(), oQ = lay.o_q(), ost = lay.o_st();
     for (int e = threadIdx.x; e < CH * XS; e += blockDim.x) b2n_sm[oX + e] = 0.0;
     const double* __restrict__ Ag = p.axesT + (size_t)cd.z * n * n;     // axesT[col*n + row] = axes[row][col]
     const double* __restrict__ Pg = p.m.lmat;                             // symmetric
@@ -971,7 +736,7 @@ __global__ void __launch_bounds__(512, 1) rwalk_mmas_kernel(const RwalkParams p,
     const int lr = lane >> 2, lc = lane & 3;
 
     // ---- helper scratch: step factor, U^(1/n), which state buffer is current, per-helper cube flags
-    const int oH = ost + CH * 4 * npad;
+    const int oH = lay.o_h();
     double* facbuf = &b2n_sm[oH];
     double* pwbuf = &b2n_sm[oH + CH];
     int* selbuf = reinterpret_cast<int*>(&b2n_sm[oH + 2 * CH]);
@@ -1241,6 +1006,88 @@ void b2n_chain_grid(const b2n_ctx* ctx, int64_t Q, int max_warps, int& chains_pe
     warps = std::max(1, std::min(max_warps, std::min(16, chains_per_cta)));
 }
 
+// The kernel of a b2n_rwalk_batch call and its launch geometry.
+enum RwalkKind { RWALK_WARP, RWALK_MMA, RWALK_WS, RWALK_MMAS };
+struct RwalkPlan {
+    RwalkKind kind;
+    int KT;                 // MMA, WS: k-tiles of 4 columns (n <= 4 KT)
+    bool plain;             // WS: affine prior and no dimension flag -- the straight-line chain phase
+    int warps;              // WARP: chains in flight per CTA, one warp each
+    int chains_per_cta;
+    size_t smem;            // dynamic shared memory, bytes
+    int ldA, ldP;           // WARP: padded column strides of axesT / the precision matrix in shared memory
+    bool ax_s, pr_s;        // WARP: axesT / the precision matrix staged in shared memory
+};
+
+// The kernel depends on the problem (model, shape, dimension flags) only, never on the queue length: a chain's result
+// must not depend on which batch it is part of -- sharded multi-GPU runs rely on that.  The queue length sets the
+// chains per CTA (and, for WARP, the warps per CTA and where the matrices live).
+//   WS   rwalk_mmaws_kernel: the precision-matrix Gaussian, ncdim == n, n in 25..32, 49..52, 57..62 -- its static
+//        schedule of the symmetric quadratic form is laid out for the largest slab count of a KT, and its draws need
+//        an idle lane 31 for the radius (n <= 62);
+//   MMA  rwalk_mma_kernel: every other registry likelihood with ncdim == n, 16 <= n <= 64;
+//   MMAS rwalk_mmas_kernel: ncdim == n > 64 when its plan fits in shared memory;
+//   WARP rwalk_kernel: everything else, and a user likelihood at every n (the lock-step kernels have no user
+//        instantiation).
+// B2N_RWALK_IMPL=warp forces WARP; B2N_RWALK_IMPL=mma forces MMA, for registry likelihoods with ncdim == n, 4 <= n <= 64.
+static int rwalk_plan(b2n_ctx* ctx, const B2nModel& m, int n, int nc, int64_t Q, const uint8_t* dimflags,
+                      RwalkPlan& pl) {
+    // warp per chain: per-warp state always; matrices (128-byte padded columns) when they fit
+    const int npad = (n + 1) & ~1;
+    const size_t per_warp = (size_t)6 * npad * sizeof(double);
+    const size_t flags_b = (size_t)((((n + 3) >> 2) << 1) + 4 * npad) * sizeof(double);
+    const size_t limit = (size_t)ctx->max_smem_optin;
+    const int max_warps = (int)std::min<size_t>(16, (limit - flags_b) / per_warp);
+    if (max_warps < 1) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the rwalk kernel");
+    const char* impl = getenv("B2N_RWALK_IMPL");
+    const bool force_warp = impl && !strcmp(impl, "warp"), force_mma = impl && !strcmp(impl, "mma");
+    const bool user = m.like_kind == B2N_LIKE_USER;
+    if (force_mma) {
+        if (user) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "B2N_RWALK_IMPL=mma: the lock-step kernels have no user-likelihood instantiation");
+        if (!(nc == n && n >= 4 && n <= 64)) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "B2N_RWALK_IMPL=mma needs ncdim == ndim <= 64");
+    }
+    pl = RwalkPlan{};
+    pl.KT = n <= 32 ? 8 : (n <= 52 ? 13 : 16);
+    pl.ldA = (nc + 15) & ~15;
+    pl.ldP = (n + 15) & ~15;
+    const bool lockstep = !force_warp && !user && nc == n;
+    if (force_mma || (lockstep && n >= 16 && n <= 64)) {
+        // matrices as register fragments, 8-chain CTAs, two resident per SM
+        const int KT = pl.KT;
+        const bool full_slabs = ((n + 7) >> 3) == (4 * KT + 7) / 8;
+        const bool ws = !force_mma && m.like_kind == B2N_LIKE_GAUSS_PREC && n <= 62 && full_slabs;
+        pl.kind = ws ? RWALK_WS : RWALK_MMA;
+        const int ctas = 2 * ctx->sm_count;
+        pl.chains_per_cta = (int)std::max<int64_t>(std::min(ctx->min_cpc, 8), (Q + ctas - 1) / ctas);
+        pl.warps = 8;
+        const int total = ws ? (KT == 8 ? MmaWsLayout<8>::TOTAL : (KT == 13 ? MmaWsLayout<13>::TOTAL : MmaWsLayout<16>::TOTAL))
+                             : (KT == 8 ? MmaLayout<8>(n).total() : (KT == 13 ? MmaLayout<13>(n).total() : MmaLayout<16>(n).total()));
+        pl.smem = (size_t)total * sizeof(double);
+        pl.plain = m.prior_kind != B2N_PRIOR_NORMAL_PPF;
+        if (dimflags)
+            for (int i = 0; i < n; i++) pl.plain = pl.plain && dimflags[i] == 0u;
+        return B2N_OK;
+    }
+    if (lockstep && n > 64 && (size_t)MmasLayout(n).total() * sizeof(double) <= limit) {
+        // large n: matrix fragments streamed from L2 (16 chains share each load), one CTA per SM
+        pl.kind = RWALK_MMAS;
+        const int ctas = ctx->sm_count;
+        pl.chains_per_cta = (int)std::max<int64_t>(std::min(ctx->min_cpc, 16), (Q + ctas - 1) / ctas);
+        pl.warps = 16;
+        pl.smem = (size_t)MmasLayout(n).total() * sizeof(double);
+        return B2N_OK;
+    }
+    pl.kind = RWALK_WARP;
+    b2n_chain_grid(ctx, Q, max_warps, pl.chains_per_cta, pl.warps);
+    const size_t fixed = per_warp * pl.warps + flags_b;
+    const size_t ax_b = (size_t)nc * pl.ldA * sizeof(double);
+    const size_t pr_b = (m.like_kind == B2N_LIKE_GAUSS_PREC) ? (size_t)n * pl.ldP * sizeof(double) : 0;
+    pl.ax_s = fixed + ax_b <= limit;
+    pl.pr_s = pr_b > 0 && fixed + (pl.ax_s ? ax_b : 0) + pr_b <= limit;
+    pl.smem = fixed + (pl.ax_s ? ax_b : 0) + (pl.pr_s ? pr_b : 0);
+    return B2N_OK;
+}
+
 extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t walks, double* u,
                                double* v, double* logl, int32_t* n_accept, int32_t* n_reject,
                                int32_t* ncall) {
@@ -1261,98 +1108,17 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     ZcScope zc(ctx);          // pinned caller buffers are read / written in place (host-pointer mode)
 
-    // shared-memory plan: per-warp state always; matrices (128-byte padded columns) when they fit
-    const int npad = (n + 1) & ~1;
-    const size_t per_warp = (size_t)6 * npad * sizeof(double);
-    const size_t flags_b = (size_t)((((n + 3) >> 2) << 1) + 4 * npad) * sizeof(double);
-    const size_t limit = (size_t)ctx->max_smem_optin;
-    const int max_warps = (int)std::min<size_t>(16, (limit - flags_b) / per_warp);
-    if (max_warps < 1) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the rwalk kernel");
-    int chains_per_cta, warps;
-    b2n_chain_grid(ctx, Q, max_warps, chains_per_cta, warps);
-    // lock-step DMMA kernel: matrices as register fragments (needs ncdim == ndim, 16 <= n <= 64
-    // and enough chains to fill CTAs).  B2N_RWALK_IMPL=warp|mma forces one of the two.
-    const char* impl = getenv("B2N_RWALK_IMPL");
-    // (the choice depends on the problem shape only, never on the queue size: a chain's result
-    // must not depend on which batch it is part of -- sharded multi-GPU runs rely on that)
-    // a user likelihood (B2N_LIKE_USER) exists only as rwalk_kernel: the warp-per-chain kernel at every n
-    const bool user = m.like_kind == B2N_LIKE_USER;
-    bool use_mma = nc == n && n >= 16 && n <= 64 && !user;
-    if (impl && !strcmp(impl, "warp")) use_mma = false;
-    if (impl && !strcmp(impl, "mma")) {
-        if (user) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "B2N_RWALK_IMPL=mma: the lock-step kernels have no user-likelihood instantiation");
-        if (!(nc == n && n >= 4 && n <= 64)) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "B2N_RWALK_IMPL=mma needs ncdim == ndim <= 64");
-        use_mma = true;
-    }
-    const int KT = n <= 32 ? 8 : (n <= 52 ? 13 : 16);
-    // direction ring depth of the lock-step kernel (B2N_RWALK_DEPTH=1: one step at a time, as before the
-    // ring; results identical)
-    int DU = 8;
-    if (const char* e = getenv("B2N_RWALK_DEPTH")) DU = (atoi(e) == 1) ? 1 : 8;
-    // draws: branch-free math, two ring items per warp at a time (default); B2N_RWALK_DRAWS=libm = libdevice
-    // log / sqrt / sincospi, one item at a time (slower; results differ by a few ulp)
-    const char* denv = getenv("B2N_RWALK_DRAWS");
-    const bool fast_draws = !(denv && !strcmp(denv, "libm")) && DU == 8;
-    const int occ = 2;                                      // 8-chain CTAs resident per SM
-    // Lock-step variants for the precision-matrix Gaussian (B2N_RWALK_WARPS forces one):
-    //   12 = rwalk_mmaws_kernel, 8 step + 4 draw warps -- the default where it applies: its static schedule of the
-    //        symmetric quadratic form is laid out for the largest slab count of a KT, and the draws need an idle lane 31
-    //        for the radius (n <= 62): n in 25..32, 49..52, 57..62;
-    //    8 = rwalk_mma_kernel (every other shape and likelihood);
-    //   16 = rwalk_mma16_kernel, sixteen warps per 8 chains (kept as a counter-example; not the default).
-    int want = 12;
-    if (const char* e = getenv("B2N_RWALK_WARPS")) want = atoi(e);
-    const bool ws_base = use_mma && n <= 62 && m.like_kind == B2N_LIKE_GAUSS_PREC && fast_draws && occ == 2;
-    const bool full_slabs = ((n + 7) >> 3) == (8 * ((4 * KT + 7) / 8)) / 8;
-    const int use_ws = (want == 12 && ws_base && full_slabs) ? 12 : 0;
-    const bool use_mma16 = want == 16 && ws_base;
-    size_t mma_smem = 0;
-    if (use_mma) {
-        const int ctas = occ * ctx->sm_count;               // 8-chain CTAs, two (three) resident per SM
-        chains_per_cta = (int)std::max<int64_t>(std::min(ctx->min_cpc, 8), (Q + ctas - 1) / ctas);
-        warps = 8;
-        const int RS = 8 * ((4 * KT + 7) / 8);
-        const int XS = RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16)), YS = RS + 2;
-        mma_smem = (size_t)(4 * npad + (((n + 3) >> 2) << 1) + DU * 8 * XS + 8 * YS + 8 * 8 + DU * 8 + 8 * 4 * npad) * sizeof(double);
-        if (use_ws)
-            mma_smem = (size_t)(KT == 8 ? MmaWsLayout<8>::TOTAL : (KT == 13 ? MmaWsLayout<13>::TOTAL : MmaWsLayout<16>::TOTAL)) * sizeof(double);
-        if (use_mma16)
-            mma_smem = (size_t)(KT == 8 ? Mma16Layout<8>::TOTAL : (KT == 13 ? Mma16Layout<13>::TOTAL : Mma16Layout<16>::TOTAL)) * sizeof(double);
-    }
-    // large n: lock-step kernel with matrix fragments streamed from L2 (16 chains share each load)
-    bool use_mmas = false;
-    int sXS = 0, sYS = 0;
-    if (!use_mma && !user && nc == n && n > 64 && !(impl && !strcmp(impl, "warp"))) {
-        const int RS = 8 * ((n + 7) / 8);
-        sXS = RS + ((RS % 16 == 4) ? 0 : ((20 - RS % 16) % 16));
-        sYS = RS + 2;
-        const size_t need = (size_t)(4 * npad + (((n + 3) >> 2) << 1) + 16 * sXS + 16 * sYS + (RS / 8) * 16 +
-                                     16 * 4 * npad + 3 * 16 + 16 * 16 / 2) * sizeof(double);      // + the helper scratch
-        if (need <= limit) {
-            use_mmas = true;
-            mma_smem = need;
-            const int ctas = ctx->sm_count;
-            chains_per_cta = (int)std::max<int64_t>(std::min(ctx->min_cpc, 16), (Q + ctas - 1) / ctas);
-            warps = 16;
-        }
-    }
-    const size_t fixed = per_warp * warps + flags_b;
-    const int ldA = (nc + 15) & ~15, ldP = (n + 15) & ~15;
-    const size_t ax_b = (size_t)nc * ldA * sizeof(double);
-    const size_t pr_b = (m.like_kind == B2N_LIKE_GAUSS_PREC) ? (size_t)n * ldP * sizeof(double) : 0;
-    const bool ax_s = fixed + ax_b <= limit;
-    const bool pr_s = pr_b > 0 && fixed + (ax_s ? ax_b : 0) + pr_b <= limit;
-    const size_t smem = (use_mma || use_mmas) ? mma_smem : fixed + (ax_s ? ax_b : 0) + (pr_s ? pr_b : 0);
-
+    RwalkPlan plan;
+    B2N_TRY(rwalk_plan(ctx, m, n, nc, Q, a->dimflags, plan));
     const bool dyn = ctx->dyn.active;        // device-paced launch (b2n_ns.cu): worklist + scalars in HBM
     if (dyn) {
-        ctx->dyn.cpc = chains_per_cta;
+        ctx->dyn.cpc = plan.chains_per_cta;
         if (ctx->dyn.plan_only) return B2N_OK;
         if (gather || ctx->ptr_mode != B2N_PTR_DEVICE) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
     }
     RwalkParams p;
     p.dyn = dyn ? ctx->dyn.dev : nullptr;
-    p.m = m; p.n = n; p.nc = nc; p.walks = walks; p.ldA = ldA; p.ldP = ldP;
+    p.m = m; p.n = n; p.nc = nc; p.walks = walks; p.ldA = plan.ldA; p.ldP = plan.ldP;
     p.loglstar = a->loglstar; p.scale = a->scale; p.seed = a->seed; p.chain0 = a->chain0;
     p.axesT = ctx->b_axesT.as<double>();
     const void *du0, *dorder, *dcta, *dfl = nullptr, *dstart = nullptr;
@@ -1371,7 +1137,7 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
     if (dyn) {
         dorder = ctx->dyn.order; dcta = ctx->dyn.cta;
     } else {
-        B2N_TRY(b2n_worklist_dev(ctx, Q, a->ell, ctx->bK, chains_per_cta, &dorder, &dcta, &ncta));
+        B2N_TRY(b2n_worklist_dev(ctx, Q, a->ell, ctx->bK, plan.chains_per_cta, &dorder, &dcta, &ncta));
     }
     std::vector<uint32_t> fl;
     if (a->dimflags) {
@@ -1399,73 +1165,54 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
     p.nacc = (int*)dna; p.nrej = (int*)dnr; p.ncall = (int*)dncl;
 
     const unsigned grid = dyn ? (unsigned)ctx->dyn.max_cta : ncta;
-#define LAUNCH(L, AXS, PRS)                                                                       \
-    do {                                                                                          \
-        B2N_TRY(b2n_func_smem(ctx, (const void*)(rwalk_kernel<L, AXS, PRS>), (size_t)(smem))); \
-        rwalk_kernel<L, AXS, PRS><<<grid, warps * 32, smem, ctx->stream>>>(p);                    \
+    const int KT = plan.KT;
+    // LAUNCH(threads, kernel): raise the kernel's shared-memory limit to the plan's, then launch it
+#define LAUNCH(THREADS, ...)                                                              \
+    do {                                                                                  \
+        B2N_TRY(b2n_func_smem(ctx, (const void*)(__VA_ARGS__), plan.smem));               \
+        __VA_ARGS__<<<grid, THREADS, plan.smem, ctx->stream>>>(p);                        \
     } while (0)
-#define CALL(L)                                                        \
-    if (ax_s && pr_s) LAUNCH(L, true, true);                           \
-    else if (ax_s) LAUNCH(L, true, false);                             \
-    else if (pr_s) LAUNCH(L, false, true);                             \
-    else LAUNCH(L, false, false);
-#define LAUNCH_MMA2(L, K, D, F)                                                                      \
-    do {                                                                                            \
-        B2N_TRY(b2n_func_smem(ctx, (const void*)(rwalk_mma_kernel<L, K, 8, D, F>), (size_t)(smem))); \
-        rwalk_mma_kernel<L, K, 8, D, F><<<grid, 256, smem, ctx->stream>>>(p);                        \
-    } while (0)
-#define LAUNCH_MMA(L, K)                        \
-    if (DU == 1) LAUNCH_MMA2(L, K, 1, false);   \
-    else if (fast_draws) LAUNCH_MMA2(L, K, 8, true); \
-    else LAUNCH_MMA2(L, K, 8, false);
-#define CALL_MMA(L)                      \
-    if (KT == 8) { LAUNCH_MMA(L, 8) }    \
-    else if (KT == 13) { LAUNCH_MMA(L, 13) } \
-    else { LAUNCH_MMA(L, 16) }
-#define CALL_MMAS(L)                                                                                  \
-    B2N_TRY(b2n_func_smem(ctx, (const void*)(rwalk_mmas_kernel<L>), (size_t)(smem)));                                                  \
-    rwalk_mmas_kernel<L><<<grid, 512, smem, ctx->stream>>>(p, sXS, sYS);
-#define LAUNCH_MMA16(K)                                                                             \
-    do {                                                                                            \
-        B2N_TRY(b2n_func_smem(ctx, (const void*)(rwalk_mma16_kernel<K>), (size_t)(smem)));          \
-        rwalk_mma16_kernel<K><<<grid, 512, smem, ctx->stream>>>(p);                                 \
-    } while (0)
-#define LAUNCH_MMAWS(K, PL)                                                                        \
-    do {                                                                                            \
-        B2N_TRY(b2n_func_smem(ctx, (const void*)(rwalk_mmaws_kernel<K, 1, PL>), (size_t)(smem)));   \
-        rwalk_mmaws_kernel<K, 1, PL><<<grid, 384, smem, ctx->stream>>>(p);                          \
-    } while (0)
+#define CALL_WARP(L)                                                                      \
+    if (plan.ax_s && plan.pr_s) LAUNCH(plan.warps * 32, rwalk_kernel<L, true, true>);     \
+    else if (plan.ax_s) LAUNCH(plan.warps * 32, rwalk_kernel<L, true, false>);            \
+    else if (plan.pr_s) LAUNCH(plan.warps * 32, rwalk_kernel<L, false, true>);            \
+    else LAUNCH(plan.warps * 32, rwalk_kernel<L, false, false>);
+#define CALL_MMA(L)                                                                       \
+    if (KT == 8) LAUNCH(256, rwalk_mma_kernel<L, 8>);                                     \
+    else if (KT == 13) LAUNCH(256, rwalk_mma_kernel<L, 13>);                              \
+    else LAUNCH(256, rwalk_mma_kernel<L, 16>);
+#define CALL_MMAS(L) LAUNCH(512, rwalk_mmas_kernel<L>);
+#define CALL_WS(K)                                                                        \
+    if (plan.plain) LAUNCH(384, rwalk_mmaws_kernel<K, true>);                             \
+    else LAUNCH(384, rwalk_mmaws_kernel<K, false>);
     B2N_TIME_BEGIN(ctx);
-    if (use_ws) {
-        // plain = no wrapped dimension and an affine prior: straight-line phase 3
-        bool plain = m.prior_kind != B2N_PRIOR_NORMAL_PPF;
-        if (a->dimflags)
-            for (int i = 0; i < n; i++) plain = plain && a->dimflags[i] == 0u;
-        if (KT == 8) { if (plain) LAUNCH_MMAWS(8, true); else LAUNCH_MMAWS(8, false); }
-        else if (KT == 13) { if (plain) LAUNCH_MMAWS(13, true); else LAUNCH_MMAWS(13, false); }
-        else { if (plain) LAUNCH_MMAWS(16, true); else LAUNCH_MMAWS(16, false); }
-    } else if (use_mma16) {
-        if (KT == 8) LAUNCH_MMA16(8);
-        else if (KT == 13) LAUNCH_MMA16(13);
-        else LAUNCH_MMA16(16);
-    } else if (use_mma) {
+    switch (plan.kind) {
+    case RWALK_WS:
+        if (KT == 8) { CALL_WS(8) }
+        else if (KT == 13) { CALL_WS(13) }
+        else { CALL_WS(16) }
+        break;
+    case RWALK_MMA:
         B2N_DISPATCH_LIKE(m.like_kind, CALL_MMA)
-    } else if (use_mmas) {
+        break;
+    case RWALK_MMAS:
         B2N_DISPATCH_LIKE(m.like_kind, CALL_MMAS)
-    } else if (user) {
-        void* args[] = {(void*)&p};
-        B2N_TRY(b2n_user_launch(ctx, a->model_id, B2N_US_RWALK + (ax_s ? 1 : 0), dim3(grid), dim3(warps * 32), smem, args));
-    } else {
-        B2N_DISPATCH_LIKE(m.like_kind, CALL)
+        break;
+    case RWALK_WARP:
+        if (m.like_kind == B2N_LIKE_USER) {
+            void* args[] = {(void*)&p};
+            B2N_TRY(b2n_user_launch(ctx, a->model_id, B2N_US_RWALK + (plan.ax_s ? 1 : 0), dim3(grid),
+                                    dim3(plan.warps * 32), plan.smem, args));
+        } else {
+            B2N_DISPATCH_LIKE(m.like_kind, CALL_WARP)
+        }
+        break;
     }
     B2N_TIME_END(ctx);
-#undef LAUNCH_MMAWS
-#undef LAUNCH_MMA16
+#undef CALL_WS
 #undef CALL_MMAS
 #undef CALL_MMA
-#undef LAUNCH_MMA
-#undef LAUNCH_MMA2
-#undef CALL
+#undef CALL_WARP
 #undef LAUNCH
     B2N_LAUNCH_CHECK(ctx);
     if (peer_on) {

@@ -1,5 +1,5 @@
-"""CPU tier: accuracy of the branch-free log / sqrt / sin-cos of csrc/b2n_fastmath.cuh (used by the rwalk
-kernels' draws when B2N_RWALK_DRAWS=fast).  The header compiles for the host too; tests/fastmath_harness.cpp
+"""CPU tier: accuracy of the branch-free log / sqrt / sin-cos of csrc/b2n_fastmath.cuh (used by the draws of the
+lock-step rwalk kernels).  The header compiles for the host too; tests/fastmath_harness.cpp
 compares it with long-double libm on the B2N uniforms (incl. arguments next to 0 and next to 1)."""
 import json
 import os

@@ -246,32 +246,13 @@ def test_rwalk_mma_matches_warp_kernel(like):
     assert 0.002 < b['n_accept'].mean() / 30 < 0.98      # (eggbox at 32-D accepts ~1 %)
 
 
-class _Warps:
-    """B2N_RWALK_WARPS for the duration of a call: 8 = lock-step kernel, 12 = warp-specialised (8 step + 4 draw
-    warps), 16 = sixteen warps per 8 chains."""
-
-    def __init__(self, w):
-        self.w = w
-
-    def __enter__(self):
-        import os
-        self.old = os.environ.get('B2N_RWALK_WARPS')
-        os.environ['B2N_RWALK_WARPS'] = str(self.w)
-
-    def __exit__(self, *a):
-        import os
-        if self.old is None:
-            os.environ.pop('B2N_RWALK_WARPS', None)
-        else:
-            os.environ['B2N_RWALK_WARPS'] = self.old
-
-
 @pytest.mark.parametrize('n,walks', [(50, 30), (62, 17), (64, 17), (32, 8), (52, 70)])
 def test_rwalk_lockstep_variants_agree(n, walks):
-    """The three lock-step kernels for the precision-matrix Gaussian -- 8 warps, 8 step + 4 draw warps (symmetric
-    quadratic form, static tile schedule: n at the largest slab count of each KT), 16 warps -- on one queue with 3
-    ellipsoids, several groups of chains per CTA and a ring that is not a multiple of 8 steps: same draws, so the same
-    accept counts (up to proposals within round-off of the threshold) and end points equal to round-off."""
+    """The lock-step kernels for the precision-matrix Gaussian -- rwalk_mma_kernel (B2N_RWALK_IMPL=mma) and the default,
+    which is the warp-specialised kernel at 32, 50, 52, 62 (symmetric quadratic form, static tile schedule: n at the
+    largest slab count of each KT) -- on one queue with 3 ellipsoids, several groups of chains per CTA and a ring that is
+    not a multiple of 8 steps: same draws, so the same accept counts (up to proposals within round-off of the threshold)
+    and end points equal to round-off."""
     from oracle import likelihoods as OL
     m = OL.gauss_corr(n, 0.4, 5.)
     dm = device_model(m)
@@ -285,34 +266,34 @@ def test_rwalk_lockstep_variants_agree(n, walks):
     Q = 5003
     u0 = good[rng.integers(len(good), size=Q)]
     ell = rng.integers(3, size=Q).astype(np.int32)
+    impls = ('mma', 'auto')
     out = {}
-    for w in (8, 12, 16):
-        with _Impl('mma'), _Warps(w):
-            out[w] = ops.rwalk_batch(dm.model_id(), u0, loglstar, 0.4, walks, 777, chain0=11, ell=ell)
-    a = out[8]
+    for impl in impls:
+        with _Impl(impl):
+            out[impl] = ops.rwalk_batch(dm.model_id(), u0, loglstar, 0.4, walks, 777, chain0=11, ell=ell)
+    a, b = out['mma'], out['auto']
     assert np.all(a['n_accept'] + a['n_reject'] == walks) and a['n_accept'].mean() > 0.05 * walks
-    for w in (12, 16):
-        b = out[w]
-        same = a['n_accept'] == b['n_accept']
-        assert same.mean() > 0.999, w
-        close(b['u'][same], a['u'][same], rtol=1e-9)
-        close(b['v'][same], a['v'][same], rtol=1e-9)
-        np.testing.assert_allclose(b['logl'][same], a['logl'][same], rtol=1e-9, atol=1e-9)
-        assert np.all(b['logl'] > loglstar) and np.all(b['n_accept'] + b['n_reject'] == walks)
+    same = a['n_accept'] == b['n_accept']
+    assert same.mean() > 0.999
+    close(b['u'][same], a['u'][same], rtol=1e-9)
+    close(b['v'][same], a['v'][same], rtol=1e-9)
+    np.testing.assert_allclose(b['logl'][same], a['logl'][same], rtol=1e-9, atol=1e-9)
+    assert np.all(b['logl'] > loglstar) and np.all(b['n_accept'] + b['n_reject'] == walks)
     # wrapped dimensions: the generic (not straight-line) chain phase of the warp-specialised kernel
     flags = ops.dimflags_from(n, [0, 3, n - 1], [5, 6])
     fo = {}
-    for w in (8, 12):
-        with _Impl('mma'), _Warps(w):
-            fo[w] = ops.rwalk_batch(dm.model_id(), u0[:777], loglstar, 0.4, walks, 778, chain0=3, ell=ell[:777], dimflags=flags)
-    same = fo[8]['n_accept'] == fo[12]['n_accept']
+    for impl in impls:
+        with _Impl(impl):
+            fo[impl] = ops.rwalk_batch(dm.model_id(), u0[:777], loglstar, 0.4, walks, 778, chain0=3, ell=ell[:777],
+                                       dimflags=flags)
+    same = fo['mma']['n_accept'] == fo['auto']['n_accept']
     assert same.mean() > 0.995
-    close(fo[12]['u'][same], fo[8]['u'][same], rtol=1e-9)
-    np.testing.assert_allclose(fo[12]['logl'][same], fo[8]['logl'][same], rtol=1e-9, atol=1e-9)
+    close(fo['auto']['u'][same], fo['mma']['u'][same], rtol=1e-9)
+    np.testing.assert_allclose(fo['auto']['logl'][same], fo['mma']['logl'][same], rtol=1e-9, atol=1e-9)
     # a start point that never moves keeps its (recomputed) v and logl in every kernel
     hi = 1e300
-    for w in (8, 12, 16):
-        with _Impl('mma'), _Warps(w):
+    for impl in impls:
+        with _Impl(impl):
             o = ops.rwalk_batch(dm.model_id(), u0[:64], hi, 0.4, 9, 5, chain0=0, ell=ell[:64])
         assert np.all(o['n_accept'] == 0)
         np.testing.assert_array_equal(o['u'], u0[:64])
