@@ -47,20 +47,43 @@ def find_decrease(samples_n):
     return ~dec, n[first - 1] if len(first) else np.empty(0, dtype=n.dtype), bounds
 
 
+def segment_plan(samples_n, approx, tile):
+    """(nseg, longest_scan) of b2n_jitter_runs' plan (jitter_plan in csrc/b2n_jitter.cu): every run of flagged samples
+    outside the stretches and every stretch is cut into segments of at most `tile` samples; a piece of a stretch scans
+    its exponentials 0..kprev (kprev = nstart for the first piece, else k of the sample before it).  longest_scan is
+    the largest kprev + 1, the most exponentials one segment scans (0 without stretches)."""
+    n = np.asarray(samples_n, dtype=np.int64)
+    N = len(n)
+    bounds = np.empty((0, 2), dtype=np.int64) if approx else find_decrease(n)[2]
+    cover = np.zeros(N + 1, dtype=np.int64)
+    np.add.at(cover, bounds[:, 0], 1)
+    np.add.at(cover, bounds[:, 1], -1)
+    edges = np.diff(np.r_[0, (np.cumsum(cover)[:N] == 0).astype(np.int64), 0])
+    runs = np.nonzero(edges == -1)[0] - np.nonzero(edges == 1)[0]
+    nseg, longest = int(np.sum(-(-runs // tile))), 0
+    for b0, b1 in bounds:
+        a = np.arange(b0, b1, tile)
+        kprev = np.where(a == b0, n[b0], n[a - 1] - 1)
+        nseg += len(a)
+        longest = max(longest, int(kprev.max()) + 1)
+    return nseg, longest
+
+
 def integrate(logl, logvol):
     """compute_integrals (utils.py:1411-1467): logwt, logz, logzvar, h."""
     from dynesty_b200.nested import _integrate
     return _integrate(np.asarray(logl, dtype=float), logvol)
 
 
-def log_t(samples_n, seed, chain, approx=False, plan=None):
-    """ln t per sample of one realisation (jitter_run, utils.py:1359-1393)."""
+def log_t(samples_n, seed, chain, approx=False, plan=None, dtype=np.float64):
+    """ln t per sample of one realisation (jitter_run, utils.py:1359-1393), computed in `dtype` from the float64
+    uniforms."""
     n = np.asarray(samples_n)
     N = len(n)
     flag, nstart, bounds = plan if plan is not None else (
         (np.ones(N, dtype=bool), np.empty(0, dtype=int), np.empty((0, 2), dtype=int)) if approx else find_decrease(n))
-    lt = np.zeros(N)
-    lt[flag] = np.log(philox.event_uniforms(seed, chain, 0, int(flag.sum()))) / n[flag]
+    lt = np.zeros(N, dtype=dtype)
+    lt[flag] = np.log(philox.event_uniforms(seed, chain, 0, int(flag.sum())).astype(dtype)) / n[flag]
     if len(nstart):
         # every stretch's exponentials at once: ticks 1..S, element e of stretch s at row s of a padded table
         m = nstart.astype(np.int64) + 1
@@ -76,7 +99,7 @@ def log_t(samples_n, seed, chain, approx=False, plan=None):
         key = np.array([int(seed) & 0xFFFFFFFF, (int(seed) >> 32) & 0xFFFFFFFF], dtype=np.uint64)
         r = philox.philox4x32_10(ctr, key)
         u = np.stack([philox.u53(r[:, 0], r[:, 1]), philox.u53(r[:, 2], r[:, 3])], axis=1)
-        y = np.ones((S, 2 * int(nb.max())))
+        y = np.ones((S, 2 * int(nb.max())), dtype=dtype)
         y[s_of, 2 * blk] = u[:, 0]
         y[s_of, 2 * blk + 1] = u[:, 1]
         y = -np.log(y[:, :W])
@@ -93,9 +116,11 @@ def log_t(samples_n, seed, chain, approx=False, plan=None):
     return lt
 
 
-def realisation(logl, samples_n, seed, chain, approx=False, logwt_ref=None, logz_ref=None, plan=None):
-    """One realisation: dict(logvol, logwt, logz, logzvar, h[, kld])."""
-    lt = log_t(samples_n, seed, chain, approx, plan)
+def realisation(logl, samples_n, seed, chain, approx=False, logwt_ref=None, logz_ref=None, plan=None,
+                dtype=np.float64):
+    """One realisation: dict(logvol, logwt, logz, logzvar, h[, kld]), in `dtype` (np.longdouble: a reference for
+    records so long that float64's running sums round at the bars the kernel is held to)."""
+    lt = log_t(samples_n, seed, chain, approx, plan, dtype)
     logvol = np.cumsum(lt)
     logwt, logz, logzvar, h = integrate(logl, logvol)
     out = dict(logvol=logvol, logwt=logwt, logz=logz, logzvar=logzvar, h=h)
@@ -106,12 +131,14 @@ def realisation(logl, samples_n, seed, chain, approx=False, logwt_ref=None, logz
     return out
 
 
-def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, arrays=False):
-    """Same contract as ``dynesty_b200.ops.jitter_runs``: the summaries (R each) and, with arrays, the R x N arrays."""
+def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, arrays=False,
+                dtype=np.float64):
+    """Same contract as ``dynesty_b200.ops.jitter_runs``: the summaries (R each) and, with arrays, the R x N arrays
+    (computed in `dtype`, returned in float64)."""
     n = np.asarray(samples_n)
     plan = (np.ones(len(n), dtype=bool), np.empty(0, dtype=int), np.empty((0, 2), dtype=int)) if approx \
         else find_decrease(n)
-    rs = [realisation(logl, n, seed, chain0 + r, approx, logwt_ref, logz_ref, plan) for r in range(R)]
+    rs = [realisation(logl, n, seed, chain0 + r, approx, logwt_ref, logz_ref, plan, dtype) for r in range(R)]
     out = dict(logz=np.array([o['logz'][-1] for o in rs]),
                logzerr=np.array([np.sqrt(max(o['logzvar'][-1], 0.)) for o in rs]),
                h=np.array([o['h'][-1] for o in rs]))
@@ -120,7 +147,19 @@ def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None
     if arrays:
         for k in ('logvol', 'logwt', 'logz') + (('kld',) if logwt_ref is not None else ()):
             out[k + '_arr'] = np.array([o[k] for o in rs])
-    return out
+    return {k: v.astype(np.float64) for k, v in out.items()}
+
+
+def expected_record(samples_n):
+    """A record with the given samples_n at its expected volumes, ln X_i = sum_{j <= i} ln(n_j / (n_j + 1)), with a
+    bounded logl whose posterior bulk sits halfway down in ln X: logl = -d/2 exp(2 ln X / d + 1), d = -ln X[-1]
+    (at least 1).  Returns dict(logl, samples_n, logvol, logwt, logz)."""
+    n = np.asarray(samples_n, dtype=np.int64)
+    logvol = np.cumsum(np.log(n / (n + 1.)))
+    d = max(-logvol[-1], 1.0)
+    logl = -0.5 * d * np.exp(2.0 * logvol / d + 1.0)
+    logwt, logz, _, _ = integrate(logl, logvol)
+    return dict(logl=logl, samples_n=n, logvol=logvol, logwt=logwt, logz=logz)
 
 
 def synthetic_record(nlive=2000, K=50, ndim=50, lnx_end=-25.0, seed=0):

@@ -1,8 +1,8 @@
-"""Generate tests/golden/jitter.npz by running the UNMODIFIED reference's jitter_run / kld_error.
+"""Generate tests/golden/jitter.npz and jitter_edges.npz by running the UNMODIFIED reference's jitter_run / kld_error.
 
 TEST INFRASTRUCTURE.  Run where the reference copy oracle/_ref exists (oracle/install_ref.py):
 
-    python -m oracle.make_golden_jitter
+    python -m oracle.make_golden_jitter [jitter] [jitter_edges]
 
 The fixture conventions are those of oracle/make_golden.py (same seed, same output directory, same oracle-backed
 stand-in for the runs whose records are used).  The draws are scripted with ``oracle.jitter.ScriptedJitterGenerator``
@@ -70,13 +70,52 @@ def gen_jitter(U):
     return out
 
 
-def main():
+def gen_jitter_edges(U):
+    """The reference's jitter_run / kld_error (approx off), driven by ScriptedJitterGenerator(SEED, JITTER_CHAIN0 + r)
+    for r = 0, 1, on two records of tests/test_jitter.py at b2n_jitter_runs' piece boundaries: [2, 1] repeated
+    JT_TILE + 1 times (one segment more than a scan tile) and one stretch JT_CHUNK + 1, .., 1 (a scan of one chunk
+    plus two exponentials).  Writes tests/golden/jitter_edges.npz: per record its logl, samples_n, logwt, logz, and
+    per realisation (the new_ keys) full logvol / logwt / logz / kld and the final logzerr and h."""
+    import sys
+    sys.path.insert(0, os.path.dirname(OUT))
+    from test_jitter import EDGES
+    names = ('pairs_Tp1', 'stretch_Cp1')
+    R = 2
+    out = dict(seed=np.int64(SEED), chain0=np.int64(JITTER_CHAIN0), r=np.arange(R), names=np.array(names))
+    for name in names:
+        rec = jitter.expected_record(EDGES[name][0])
+        p = 'edge_%s_' % name
+        out.update({p + k: rec[k] for k in ('logl', 'samples_n', 'logwt', 'logz')})
+        N = len(rec['logl'])
+        res = U.Results(dict(samples_u=np.zeros((N, 1)), samples=np.zeros((N, 1)), samples_id=np.zeros(N, dtype=int),
+                             logl=rec['logl'], samples_n=rec['samples_n'], logvol=rec['logvol'], logwt=rec['logwt'],
+                             logz=rec['logz'], logzerr=np.zeros(N), information=np.zeros(N)))
+        cols = {k: [] for k in ('logvol', 'logwt', 'logz', 'kld', 'logzerr', 'h')}
+        for r in range(R):
+            rs = jitter.ScriptedJitterGenerator(SEED, JITTER_CHAIN0 + r)
+            kld, new = U.kld_error(res, 'jitter', rstate=rs, return_new=True, approx=False)
+            for k in ('logvol', 'logwt', 'logz'):
+                cols[k].append(np.asarray(new[k]))
+            cols['kld'].append(kld)
+            cols['logzerr'].append(new['logzerr'][-1])
+            cols['h'].append(U.compute_integrals(logl=rec['logl'], logvol=new['logvol'])[3][-1])
+        out.update({p + 'new_' + k: np.array(v) for k, v in cols.items()})
+    np.savez_compressed(os.path.join(OUT, 'jitter_edges.npz'), **out)
+    return out
+
+
+def main(argv=()):
+    """All fixtures, or only those named on the command line (jitter, jitter_edges)."""
     os.makedirs(OUT, exist_ok=True)
     refshim.import_reference()
     from dynesty import utils as U
-    gen_jitter(U)
-    print('wrote', os.path.join(OUT, 'jitter.npz'), os.path.getsize(os.path.join(OUT, 'jitter.npz')))
+    for name, gen in (('jitter', gen_jitter), ('jitter_edges', gen_jitter_edges)):
+        if not argv or name in argv:
+            gen(U)
+            f = os.path.join(OUT, name + '.npz')
+            print('wrote', f, os.path.getsize(f))
 
 
 if __name__ == '__main__':
-    main()
+    import sys
+    main(sys.argv[1:])

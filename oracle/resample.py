@@ -73,16 +73,17 @@ def reference_counts(logl, strand, lower, m):
     return inside.astype(np.int64) @ m
 
 
-def realisation(logl, strand, m, counts, end=None, logwt_ref=None, logz_ref=None):
+def realisation(logl, strand, m, counts, end=None, logwt_ref=None, logz_ref=None, dtype=np.float64):
     """One realisation from its multiplicities and the live counts of the record's samples: dict(idx, samples_n,
-    logvol, logwt, logz, logzvar, h[, kld])."""
+    logvol, logwt, logz, logzvar, h[, kld]), in `dtype` (np.longdouble: a reference for records so long that float64's
+    running sums round at the bars the kernel is held to)."""
     from dynesty_b200.nested import _integrate
     logl = np.asarray(logl, dtype=float)
     ms = m[strand]
     idx = np.repeat(np.arange(len(logl)), ms)
     copy = np.arange(len(idx)) - np.repeat(np.cumsum(ms) - ms, ms)
     n = counts[idx] - (copy * np.asarray(end)[idx] if end is not None else 0)
-    logvol = np.cumsum(np.log(n / (n + 1.)))
+    logvol = np.cumsum(np.log(n.astype(dtype) / (n + 1)))
     logwt, logz, logzvar, h = _integrate(logl[idx], logvol)
     out = dict(idx=idx, samples_n=n, logvol=logvol, logwt=logwt, logz=logz, logzvar=logzvar, h=h)
     if logwt_ref is not None:
@@ -102,8 +103,8 @@ def csr_counts(strand, piece_ptr, piece_strand, m):
 
 
 def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, chain0=0, logwt_ref=None, logz_ref=None,
-                  multiplicities=False):
-    """Same contract as ``dynesty_b200.ops.resample_runs``."""
+                  multiplicities=False, dtype=np.float64):
+    """Same contract as ``dynesty_b200.ops.resample_runs`` (computed in `dtype`, returned in float64)."""
     strand = np.asarray(strand, dtype=np.int64)
     base = np.asarray(base, dtype=bool)
     piece_strand = np.asarray(piece_strand, dtype=np.int64)
@@ -112,13 +113,13 @@ def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, cha
     for r in range(R):
         m = draw_multiplicities(base, seed, chain0 + r)
         c = csr_counts(strand, piece_ptr, piece_strand, m)
-        rs.append(realisation(logl, strand, m, c, end, logwt_ref, logz_ref))
+        rs.append(realisation(logl, strand, m, c, end, logwt_ref, logz_ref, dtype))
         ms.append(m)
-    out = dict(logz=np.array([o['logz'][-1] for o in rs]),
-               logzerr=np.array([np.sqrt(max(o['logzvar'][-1], 0.)) for o in rs]),
-               h=np.array([o['h'][-1] for o in rs]))
+    out = dict(logz=np.array([o['logz'][-1] for o in rs], dtype=np.float64),
+               logzerr=np.array([np.sqrt(max(o['logzvar'][-1], 0.)) for o in rs], dtype=np.float64),
+               h=np.array([o['h'][-1] for o in rs], dtype=np.float64))
     if logwt_ref is not None:
-        out['kld'] = np.array([o['kld'][-1] for o in rs])
+        out['kld'] = np.array([o['kld'][-1] for o in rs], dtype=np.float64)
     if multiplicities:
         out['mult'] = np.array(ms).reshape(R, S)
     return out

@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 
 from oracle import jitter as OJ
-from dynesty_b200 import dynamic as D, likelihoods as DL, ops, replicas, utils as DU
+from dynesty_b200 import _lib, dynamic as D, likelihoods as DL, ops, replicas, utils as DU
+from test_jitter import EDGES, JT_CHUNK, JT_TILE
 
 pytestmark = pytest.mark.gpu
 
@@ -48,6 +49,20 @@ def _oracle(records, name, approx):
     return _oracle_cache[name, approx]
 
 
+def _compare(o, ref, rows=slice(None)):
+    """Realisations `rows` of the kernel's output o against the oracle's ref (the same realisations, in order)."""
+    for k in ('logz', 'logzerr', 'h', 'kld'):
+        np.testing.assert_allclose(o[k][rows], ref[k], rtol=1e-9, atol=0, err_msg=k)
+    for k in ('logvol', 'logz'):
+        np.testing.assert_allclose(o[k + '_arr'][rows], ref[k + '_arr'], rtol=0, atol=1e-9, err_msg=k)
+    # logwt is compared through the importance weights it defines: where ln t is within a few ulps of 0 (U next to 1),
+    # numpy's dlogvol = diff(cumsum(ln t)) inside log1p(-exp(dlogvol)) has a large relative rounding error, which the
+    # kernel (it uses ln t itself) does not; those samples carry no weight
+    np.testing.assert_allclose(np.exp(o['logwt_arr'][rows] - o['logz'][rows, None]),
+                               np.exp(ref['logwt_arr'] - ref['logz'][:, None]), rtol=0, atol=1e-12)
+    np.testing.assert_allclose(o['kld_arr'][rows], ref['kld_arr'], rtol=0, atol=1e-9)
+
+
 @pytest.mark.parametrize('R', [1, 7, 128])
 @pytest.mark.parametrize('approx', [False, True])
 @pytest.mark.parametrize('name', ['golden', 'c2', 'dyn'])
@@ -55,20 +70,71 @@ def test_kernel_matches_oracle(records, name, approx, R):
     logl, n, wt, z = records[name]
     o = ops.jitter_runs(logl, n, R, SEED, chain0=CHAIN0, approx=approx, logwt_ref=wt, logz_ref=z, arrays=True)
     ref = _oracle(records, name, approx)
-    for k in ('logz', 'logzerr', 'h', 'kld'):
-        np.testing.assert_allclose(o[k], ref[k][:R], rtol=1e-9, atol=0, err_msg=k)
-    for k in ('logvol', 'logz'):
-        np.testing.assert_allclose(o[k + '_arr'], ref[k + '_arr'][:R], rtol=0, atol=1e-9, err_msg=k)
-    # logwt is compared through the importance weights it defines: where ln t is within a few ulps of 0 (U next to 1),
-    # numpy's dlogvol = diff(cumsum(ln t)) inside log1p(-exp(dlogvol)) has a large relative rounding error, which the
-    # kernel (it uses ln t itself) does not; those samples carry no weight
-    np.testing.assert_allclose(np.exp(o['logwt_arr'] - o['logz'][:, None]),
-                               np.exp(ref['logwt_arr'][:R] - ref['logz'][:R, None]), rtol=0, atol=1e-12)
-    np.testing.assert_allclose(o['kld_arr'], ref['kld_arr'][:R], rtol=0, atol=1e-9)
+    _compare(o, {k: v[:R] for k, v in ref.items()})
     # the summary-only path computes the same numbers
     s = ops.jitter_runs(logl, n, R, SEED, chain0=CHAIN0, approx=approx, logwt_ref=wt, logz_ref=z)
     for k in ('logz', 'logzerr', 'h', 'kld'):
         assert np.array_equal(s[k], o[k]), k
+
+
+def _run_both(rec, R, approx, seed=SEED, chain0=CHAIN0, dtype=np.float64):
+    """The kernel's R realisations (full arrays) and the oracle's (computed in dtype)."""
+    args = (rec['logl'], rec['samples_n'], R, seed)
+    kw = dict(chain0=chain0, approx=approx, logwt_ref=rec['logwt'], logz_ref=rec['logz'][-1], arrays=True)
+    return ops.jitter_runs(*args, **kw), OJ.jitter_runs(*args, dtype=dtype, **kw)
+
+
+@pytest.mark.parametrize('approx', [False, True])
+@pytest.mark.parametrize('name', list(EDGES))
+def test_kernel_matches_oracle_at_plan_edges(name, approx):
+    """Records at the segment tiles of the scan kernels, the chunks of a stretch piece's scan and the tiles of flagged
+    samples (tests/test_jitter.py): every carry from one piece to the next is used."""
+    n, plan = EDGES[name]
+    assert OJ.segment_plan(n, approx, JT_TILE) == plan[approx]
+    # flat: numpy's float64 running sums over its 2^20 + 1 samples are off by 6.5e-10 in kld (0.44) against the same
+    # oracle in long double, the whole gap to the kernel; the long double oracle keeps the bars
+    o, ref = _run_both(OJ.expected_record(n), 2, approx, dtype=np.longdouble if name == 'flat' else np.float64)
+    _compare(o, ref)
+
+
+@pytest.mark.parametrize('approx', [False, True])
+@pytest.mark.parametrize('shape', ['c2', 'c4'])
+def test_kernel_matches_oracle_on_real_run_sizes(shape, approx):
+    """A C2-shaped record run to ln X = -30 (more segments than a scan tile) and a C4-shaped one (nlive 8000, K 400,
+    ln X -> -100: more segments than a tile and an add_live tail scanning several chunks); the oracle on two of 16
+    realisations."""
+    nlive, K, lnx = {'c2': (2000, 50, -30.), 'c4': (8000, 400, -100.)}[shape]
+    logl, n = OJ.synthetic_record(nlive, K, lnx_end=lnx)
+    nseg, scan = OJ.segment_plan(n, approx, JT_TILE)
+    if not approx:
+        assert nseg > JT_TILE and (shape == 'c2' or scan > JT_CHUNK)
+    wt, lz = OJ.integrate(logl, np.cumsum(np.log(n / (n + 1.))))[:2]
+    z = lz[-1]
+    o = ops.jitter_runs(logl, n, 16, SEED, chain0=CHAIN0, approx=approx, logwt_ref=wt, logz_ref=z, arrays=True)
+    for r in (0, 15):
+        ref = OJ.jitter_runs(logl, n, 1, SEED, CHAIN0 + r, approx, wt, z, arrays=True)
+        _compare(o, ref, slice(r, r + 1))
+
+
+@pytest.mark.parametrize('approx', [False, True])
+def test_kernel_matches_oracle_at_stream_limits(approx):
+    """Chain ids crossing into their high word, a seed with bits above 32 set, and the largest R on a one-segment
+    record; R = 65536 is refused before anything is launched."""
+    rec = OJ.expected_record(np.r_[np.full(40, 30), np.arange(50, 0, -1)])
+    _compare(*_run_both(rec, 4, approx, chain0=2 ** 32 - 2))
+    _compare(*_run_both(rec, 3, approx, seed=(0x9E3779B9 << 32) | 12345))
+    one = OJ.expected_record([6, 5, 4, 3, 2, 1])
+    assert OJ.segment_plan(one['samples_n'], approx, JT_TILE)[0] == 1
+    args = (one['logl'], one['samples_n'])
+    kw = dict(approx=approx, logwt_ref=one['logwt'], logz_ref=one['logz'][-1], arrays=True)
+    o = ops.jitter_runs(*args, 65535, SEED, chain0=CHAIN0, **kw)
+    for r in (0, 65534):
+        _compare(o, OJ.jitter_runs(*args, 1, SEED, chain0=CHAIN0 + r, **kw), slice(r, r + 1))
+    ctx = _lib.default_context()
+    launches = ctx.launch_count()
+    with pytest.raises(ValueError):
+        ops.jitter_runs(*args, 65536, SEED, chain0=CHAIN0, **kw)
+    assert ctx.launch_count() == launches
 
 
 @pytest.mark.parametrize('approx', [False, True])

@@ -8,9 +8,10 @@ import numpy as np
 import pytest
 
 from oracle import nsstrands, resample as OR
-from dynesty_b200 import dynamic as D, likelihoods as DL, nested as N, ops, replicas, utils as DU
+from dynesty_b200 import _lib, dynamic as D, likelihoods as DL, nested as N, ops, replicas, utils as DU
 from dynesty_b200.nested import Results
 from test_gpu_nsloop import _bound, _live, _models
+from test_resample import RECORDS as TILE_RECORDS, RS_TILE, host_record
 
 pytestmark = pytest.mark.gpu
 
@@ -164,11 +165,18 @@ def records(gold, dyn_record):
     return out
 
 
-def _oracle(res, R, chain0=CHAIN0):
+def _oracle(res, R, chain0=CHAIN0, seed=SEED, dtype=np.float64):
     plan = DU.strand_plan(res)
     pp, ps = DU._piece_csr(res['logl'], plan)
-    return OR.resample_runs(res['logl'], plan['strand'], plan['base'], pp, ps, plan['end'], R, SEED, chain0,
-                            res['logwt'], res['logz'][-1], multiplicities=True)
+    return OR.resample_runs(res['logl'], plan['strand'], plan['base'], pp, ps, plan['end'], R, seed, chain0,
+                            res['logwt'], res['logz'][-1], multiplicities=True, dtype=dtype)
+
+
+def _compare(o, ref, rows=slice(None)):
+    """Realisations `rows` of the kernel's output o against the oracle's ref (the same realisations, in order)."""
+    assert np.array_equal(o['mult'][rows], ref['mult'])
+    for k in ('logz', 'logzerr', 'h', 'kld'):
+        np.testing.assert_allclose(o[k][rows], ref[k], rtol=1e-9, atol=1e-12, err_msg=k)
 
 
 _cache = {}
@@ -182,9 +190,55 @@ def test_kernel_matches_oracle(records, name, R):
         _cache[name] = _oracle(res, 128)
     ref = _cache[name]
     o = DU.resample_realisations(res, R, SEED, CHAIN0, multiplicities=True)
-    assert np.array_equal(o['mult'], ref['mult'][:R])
-    for k in ('logz', 'logzerr', 'h', 'kld'):
-        np.testing.assert_allclose(o[k], ref[k][:R], rtol=1e-9, atol=1e-12, err_msg=k)
+    _compare(o, {k: v[:R] for k, v in ref.items()})
+
+
+@pytest.mark.parametrize('name', list(TILE_RECORDS))
+def test_kernel_matches_oracle_at_tile_edges(name):
+    """Records at resample_scan_kernel's tile boundaries (tests/test_resample.py)."""
+    res = TILE_RECORDS[name]
+    _check_identity(res)
+    ref = _oracle(res, 16)
+    if name == 'long_run':
+        # realisations without slot 0: whole tiles with no present sample between present ones; and without slot 1:
+        # the first sample is absent
+        assert (ref['mult'][:, 0] == 0).any() and (ref['mult'][:, 1] == 0).any()
+    _compare(DU.resample_realisations(res, 16, SEED, CHAIN0, multiplicities=True), ref)
+
+
+def test_kernel_matches_oracle_without_the_final_live_points():
+    """The C2-shaped record cut before its add_live tail: the live points' open pieces run to the end of the record,
+    across tiles."""
+    full = OR.synthetic_strand_record()
+    nd = int(full['niter'])
+    res = Results({k: v[:nd] if isinstance(v, np.ndarray) else v for k, v in full.items()})
+    plan = DU.strand_plan(res)
+    assert plan['end'] is None and (plan['open'] < nd - RS_TILE).any()
+    _compare(DU.resample_realisations(res, 4, SEED, CHAIN0, multiplicities=True), _oracle(res, 4))
+
+
+def test_kernel_matches_oracle_on_c4_sized_record():
+    """nlive 8000, K 400, ln X -> -100 (808k samples): numpy's float64 running sums are off by 2.7e-11 in kld (3.6e-4)
+    against the same oracle in long double, the whole gap to the kernel; the long double oracle keeps the bars."""
+    res = Results(OR.synthetic_strand_record(8000, 400, lnx_end=-100.))
+    _compare(DU.resample_realisations(res, 2, SEED, CHAIN0, multiplicities=True), _oracle(res, 2, dtype=np.longdouble))
+
+
+def test_kernel_matches_oracle_at_stream_limits():
+    """Chain ids crossing into their high word, a seed with bits above 32 set, and the largest R on a one-tile record;
+    R = 65536 is refused before anything is launched."""
+    res = host_record(np.random.default_rng(5).integers(0, 20, 200), 20)
+    _compare(DU.resample_realisations(res, 4, SEED, 2 ** 32 - 2, multiplicities=True), _oracle(res, 4, 2 ** 32 - 2))
+    seed = (0x9E3779B9 << 32) | 12345
+    _compare(DU.resample_realisations(res, 3, seed, CHAIN0, multiplicities=True), _oracle(res, 3, CHAIN0, seed))
+    o = DU.resample_realisations(res, 65535, SEED, CHAIN0, multiplicities=True)
+    for r in (0, 65534):
+        _compare(o, _oracle(res, 1, CHAIN0 + r), slice(r, r + 1))
+    ctx = _lib.default_context()
+    launches = ctx.launch_count()
+    with pytest.raises(ValueError):
+        DU.resample_realisations(res, 65536, SEED, CHAIN0)
+    assert ctx.launch_count() == launches
 
 
 def test_kernel_matches_reference_fixture(gold, records):

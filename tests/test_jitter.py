@@ -1,8 +1,10 @@
 """CPU tier: run uncertainties from simulated prior volumes.  The numpy restatement (oracle/jitter.py) against the
 reference's own jitter_run / kld_error / _find_decrease (recorded in tests/golden/jitter.npz by oracle/make_golden_jitter.py,
-driven by ScriptedJitterGenerator on the same B2N streams), the stopping function's argument handling, and a dynamic run on
+driven by ScriptedJitterGenerator on the same B2N streams; tests/golden/jitter_edges.npz for records at the kernel's piece
+boundaries), the kernel's segment plan on those records, the stopping function's argument handling, and a dynamic run on
 the oracle backend that stops on the evidence error."""
 import os
+import re
 import warnings
 
 import numpy as np
@@ -12,7 +14,54 @@ from oracle import jitter as OJ, philox
 from dynesty_b200 import dynamic as D, likelihoods as DL, ops, utils as DU
 from dynesty_b200.nested import Results
 
-GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'jitter.npz')
+HERE = os.path.dirname(os.path.abspath(__file__))
+GOLDEN = os.path.join(HERE, 'golden', 'jitter.npz')
+GOLDEN_EDGES = os.path.join(HERE, 'golden', 'jitter_edges.npz')
+CSRC = os.path.join(os.path.dirname(HERE), 'dynesty_b200', 'csrc')
+
+
+def csrc_constant(fname, name):
+    """`constexpr int name = value;` of a kernel source: the records below are built from the kernels' own tile sizes,
+    so that they keep straddling the boundaries when a size changes."""
+    with open(os.path.join(CSRC, fname)) as f:
+        m = re.search(r'constexpr\s+int\s+%s\s*=\s*(\d+)\s*;' % name, f.read())
+    assert m, '%s not found in %s' % (name, fname)
+    return int(m.group(1))
+
+
+JT_TILE = csrc_constant('b2n_jitter.cu', 'JT_TILE')      # samples per segment, segments per scan tile
+JT_CHUNK = csrc_constant('b2n_jitter.cu', 'JT_CHUNK')    # exponentials per step of a stretch piece's scan
+
+
+def _cdiv(a, b):
+    return -(-a // b)
+
+
+def _edges():
+    """Records at b2n_jitter_runs' piece boundaries: name -> (samples_n, {approx: segment_plan}).  T = JT_TILE,
+    C = JT_CHUNK.
+      pairs_*    [2, 1] repeated: that many two-sample stretches, one segment each (the scan kernels' tiles of T);
+      flat       T^2 + 1 flagged samples: T + 1 segments in both modes;
+      stretch_*  one stretch nstart, .., 1: a scan of nstart + 1 exponentials (chunks of C), pieces of T samples;
+      run_*      a run of flagged samples (tiles of T) right before a stretch;
+      n1, n2*    the smallest records."""
+    T, C = JT_TILE, JT_CHUNK
+    out = {}
+    for tag, k in (('Tm1', T - 1), ('T', T), ('Tp1', T + 1), ('2Tp1', 2 * T + 1)):
+        out['pairs_' + tag] = (np.tile([2, 1], k), {False: (k, 3), True: (_cdiv(2 * k, T), 0)})
+    out['flat'] = (np.full(T * T + 1, 500), {False: (T + 1, 0), True: (T + 1, 0)})
+    for tag, s in (('Cm1', C - 1), ('C', C), ('Cp1', C + 1), ('2C', 2 * C), ('8000', 8000)):
+        out['stretch_' + tag] = (np.arange(s, 0, -1), {False: (_cdiv(s, T), s + 1), True: (_cdiv(s, T), 0)})
+    for tag, L in (('Tm1', T - 1), ('T', T), ('Tp1', T + 1)):
+        out['run_' + tag] = (np.r_[np.full(L, 100), np.arange(200, 0, -1)],
+                             {False: (_cdiv(L, T) + 1, 201), True: (_cdiv(L + 200, T), 0)})
+    out['n1'] = (np.array([7]), {False: (1, 0), True: (1, 0)})
+    out['n2'] = (np.array([2, 1]), {False: (1, 3), True: (1, 0)})
+    out['n2flat'] = (np.array([4, 4]), {False: (1, 0), True: (1, 0)})
+    return out
+
+
+EDGES = _edges()
 
 
 @pytest.fixture(scope='module')
@@ -58,6 +107,49 @@ def test_oracle_realisations_equal_reference(jit, name, approx):
         for k in ('logvol', 'logwt', 'logz'):
             np.testing.assert_allclose(o[k + '_arr'][r], jit[q + k][i], rtol=1e-12, atol=1e-12, err_msg=k)
         np.testing.assert_allclose(o['kld_arr'][r], jit[q + 'kld'][i], rtol=0, atol=1e-13)
+
+
+@pytest.mark.parametrize('name', list(EDGES))
+def test_segment_plan_of_edge_records(name):
+    n, plan = EDGES[name]
+    for approx in (False, True):
+        assert OJ.segment_plan(n, approx, JT_TILE) == plan[approx], approx
+
+
+def test_segment_plan_of_synthetic_records():
+    T = JT_TILE
+    # [3, 2, 1 | 13 | 13, 12 | 23, 22]: stretches of 3, 2, 2 samples around one flagged sample
+    assert OJ.segment_plan([3, 2, 1, 13, 13, 12, 23, 22], False, 2) == (5, 24)
+    assert OJ.segment_plan([3, 2, 1, 13, 13, 12, 23, 22], True, 2) == (4, 0)
+    # rounds of K (one stretch each, K < T), then the add_live tail nlive, .., 1 in pieces of T
+    for (nlive, K, lnx), nrounds in (((2000, 50, -25.), 1000), ((2000, 50, -30.), 1200), ((8000, 400, -100.), 2000)):
+        n = OJ.synthetic_record(nlive, K, lnx_end=lnx)[1]
+        assert len(n) == nrounds * K + nlive
+        assert OJ.segment_plan(n, False, T) == (nrounds + _cdiv(nlive, T), nlive + 1)
+        assert OJ.segment_plan(n, True, T) == (_cdiv(len(n), T), 0)
+    # the sizes a real run reaches straddle both boundaries: more than T segments, more than C exponentials
+    assert OJ.segment_plan(OJ.synthetic_record(2000, 50, lnx_end=-30.)[1], False, T)[0] > T
+    assert OJ.segment_plan(OJ.synthetic_record(8000, 400, lnx_end=-100.)[1], False, T)[1] > JT_CHUNK
+
+
+def test_oracle_realisations_equal_reference_at_plan_edges():
+    """The reference's own jitter_run / kld_error on two records at the kernel's piece boundaries (recorded by
+    oracle/make_golden_jitter.py): more stretches than a scan tile holds, and a stretch scanning one exponential
+    more than a chunk."""
+    g = dict(np.load(GOLDEN_EDGES))
+    for name in g['names']:
+        p = 'edge_%s_' % name
+        q = p + 'new_'
+        o = OJ.jitter_runs(g[p + 'logl'], g[p + 'samples_n'], len(g['r']), int(g['seed']), int(g['chain0']), False,
+                           g[p + 'logwt'], g[p + 'logz'][-1], arrays=True)
+        for i in range(len(g['r'])):
+            for k in ('logz', 'kld'):
+                np.testing.assert_allclose(o[k][i], g[q + k][i][-1], rtol=1e-12, atol=0, err_msg=k)
+            for k in ('logzerr', 'h'):
+                np.testing.assert_allclose(o[k][i], g[q + k][i], rtol=1e-12, atol=0, err_msg=k)
+            for k in ('logvol', 'logwt', 'logz'):
+                np.testing.assert_allclose(o[k + '_arr'][i], g[q + k][i], rtol=1e-12, atol=1e-12, err_msg=k)
+            np.testing.assert_allclose(o['kld_arr'][i], g[q + 'kld'][i], rtol=0, atol=1e-13)
 
 
 def test_scripted_generator_beta_and_exponential_are_single_events():

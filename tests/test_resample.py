@@ -7,13 +7,55 @@ import os
 import numpy as np
 import pytest
 
-from oracle import nsstrands, resample as OR
+from oracle import jitter as OJ, nsstrands, resample as OR
 from dynesty_b200 import dynamic as D, likelihoods as DL, nested as N, ops, utils as DU
 from dynesty_b200.nested import Results
+from test_jitter import csrc_constant
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'resample.npz')
 NAMES = ['host', 'dev', 'devnolive', 'dyn']
 KEYS = ('logl', 'samples_id', 'samples_it', 'samples_n', 'logwt', 'logz', 'logvol', 'ncall_per_it', 'samples_batch')
+RS_TILE = csrc_constant('b2n_resample.cu', 'RS_TILE')    # samples per tile of resample_scan_kernel
+
+
+def host_record(slots, nlive, logl=None):
+    """A static record of a host loop (one removal per iteration): the dead points come from the live slots `slots`
+    in order, then the nlive final live points (slots 0..nlive-1).  Every point is born right above the point its
+    slot lost before it.  logl: rising along the record (default: oracle.jitter.expected_record's); logwt and logz
+    are those of the expected volumes."""
+    slots = np.asarray(slots, dtype=np.int64)
+    ids = np.r_[slots, np.arange(nlive)]
+    its = np.zeros(len(ids), dtype=np.int64)
+    last = {}
+    for i, s in enumerate(ids):
+        its[i] = last.get(s, -1) + 1
+        last[s] = i
+    n = np.r_[np.full(len(slots), nlive), np.arange(nlive, 0, -1)]
+    rec = OJ.expected_record(n)
+    if logl is not None:
+        rec['logl'] = np.asarray(logl, dtype=float)
+        rec['logwt'], rec['logz'] = OJ.integrate(rec['logl'], rec['logvol'])[:2]
+    return Results(dict(rec, samples_id=ids, samples_it=its, niter=len(slots)))
+
+
+def _records():
+    """Records at resample_scan_kernel's tile boundaries (R = RS_TILE):
+      long_run  nlive 3: two slots die twice, then slot 0 more than 2R times in a row, then the final live points --
+                a realisation that does not draw slot 0 has whole tiles without a present sample after present ones;
+      N_*       N = R - 1, R, R + 1 (nlive 400: the tile boundary falls in the add_live tail, which carries weight);
+      N1        one sample, one strand."""
+    T = RS_TILE
+    rng = np.random.default_rng(3)
+    out = {}
+    slots = np.r_[[1, 2, 1, 2], np.zeros(2 * T + 300, dtype=np.int64)]
+    out['long_run'] = host_record(slots, 3, logl=np.linspace(-5.0, 0.0, len(slots) + 3))
+    for tag, N in (('Tm1', T - 1), ('T', T), ('Tp1', T + 1)):
+        out['N_' + tag] = host_record(rng.integers(0, 400, N - 400), 400)
+    out['N1'] = host_record([], 1)
+    return out
+
+
+RECORDS = _records()
 
 
 @pytest.fixture(scope='module')
@@ -126,6 +168,26 @@ def test_reference_rule_misses_device_round_counts(strand_ops):
     # every slot counted as occupied: nlive everywhere instead of the saw-tooth nlive - j
     assert (ref[:h] == 40).all() and (res.samples_n[:h] < 40).sum() >= h * 3 // 5
     assert np.array_equal(_identity(res)['samples_n'], res.samples_n)
+
+
+@pytest.mark.parametrize('name', list(RECORDS))
+def test_tile_edge_records_are_consistent(name):
+    """The hand-built records: the piece rule with every multiplicity 1 gives back samples_n, and they sit where their
+    names say."""
+    res = RECORDS[name]
+    plan = _check_strands(res, int(res.samples_n[int(res.niter)]))           # the first final live point: nlive
+    assert np.array_equal(_identity(res)['samples_n'], res.samples_n)
+    pp, ps = DU._piece_csr(res.logl, plan)
+    assert np.array_equal(OR.csr_counts(plan['strand'], pp, ps, np.ones(len(plan['ids']), dtype=np.int64)),
+                          res.samples_n)
+    N = len(res.logl)
+    if name == 'long_run':
+        ids = res.samples_id
+        run = np.nonzero(ids == 0)[0][:-1]
+        assert len(run) > 2 * RS_TILE and np.array_equal(run, np.arange(4, 4 + len(run)))
+        assert set(ids[:4]) == {1, 2}
+    else:
+        assert N == {'N_Tm1': RS_TILE - 1, 'N_T': RS_TILE, 'N_Tp1': RS_TILE + 1, 'N1': 1}[name]
 
 
 # ---------------------------------------------------------------------------------------------- strand records
