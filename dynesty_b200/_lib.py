@@ -126,6 +126,7 @@ SYMBOLS = {
     'b2n_ns_set_live_it': (C.c_int, [_P, _P]),
     'b2n_ns_get_live_it': (C.c_int, [_P, _P]),
     'b2n_resample_runs': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _P, _P, _P, _P]),
+    'b2n_merge_runs': (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

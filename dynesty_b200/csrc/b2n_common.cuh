@@ -168,6 +168,10 @@ void b2n_ns_release(b2n_ctx* ctx);
 void b2n_friends_release(b2n_ctx* ctx);
 int b2n_bound_set_dev(b2n_ctx* ctx, int K, int nc, const double* dctrs, const double* dams, const double* daxes,
                       const double* h_logvols);
+// compute_integrals of one record with given ln t per sample, on the passes of b2n_jitter_runs (b2n_jitter.cu).
+// Device pointers; uses ctx->scratch0 / scratch1; does not synchronise.
+int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
+                      double* logwt, double* logz, double* logzvar, double* h);
 
 // gather-mode plumbing shared by the chain entry points (b2n_peer.cu).  b2n_peer_begin: when
 // gather mode is on, point the 7 output arrays at this rank's rows of its own window and fill

@@ -18,7 +18,11 @@
 //   pass 2   (segments x R)  logvol, logwt, logz per sample; segment sums of the h increments (A), of dh * dlogvol (C)
 //                            and of the KL terms (K); the full arrays when asked for
 //   scan 2   (R)             logzerr[-1], h[-1], kld[-1]; the kld prefix at every segment start
-//   offsets  (segments x R)  adds that prefix to the full kld array (only when it is asked for)
+//   offsets  (segments x R)  adds that prefix to the full kld array (only when it is asked for), and the prefixes of
+//                            A and C to the full h and logzvar arrays (b2n_integrate_lnt only)
+//
+// b2n_integrate_lnt (below, for b2n_merge.cu) runs the same passes in a deterministic mode: one realisation whose ln t
+// per sample is read from an array (segment_lnt<true>), over a plan of tick-0 segments only.
 #include "b2n_device.cuh"
 
 #include <algorithm>
@@ -43,6 +47,7 @@ struct JArgs {
     const int32_t* nlive;    // samples_n
     const int32_t* aux;      // flagged sample: its element of the tick-0 event; stretch sample: k = samples_n - 1
     const JSeg* seg;
+    const double* lnt;       // given ln t per sample (b2n_integrate_lnt), else NULL
     int64_t N, nseg;
     int R;
     double zref;
@@ -51,6 +56,7 @@ struct JArgs {
     double* zend;            // R: logz[-1]
     double* out_logz; double* out_logzerr; double* out_h; double* out_kld;                // R each, may be NULL
     double* f_logvol; double* f_logwt; double* f_logz; double* f_kld;                     // R x N, may be NULL
+    double* f_h; double* f_logzvar;                      // N, may be NULL (b2n_integrate_lnt only)
 };
 
 __device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
@@ -106,7 +112,13 @@ __device__ double block_scan(double* x, int n, double* wsum, Op op) {
 }
 
 // ln t of the segment's samples into lt[0, len)
+template <bool GIVEN>
 __device__ void segment_lnt(const JArgs& A, const JSeg& s, int r, double* lt, double* cap, double* buf, double* wsum) {
+    if (GIVEN) {
+        for (int i = threadIdx.x; i < s.len; i += blockDim.x) lt[i] = A.lnt[s.a + i];
+        __syncthreads();
+        return;
+    }
     ChainRng g;
     g.init(A.seed, A.chain0 + (uint64_t)r);
     const int L = s.len;
@@ -135,7 +147,9 @@ __device__ void segment_lnt(const JArgs& A, const JSeg& s, int r, double* lt, do
     __syncthreads();
 }
 
-template <int PASS>
+// GIVEN: ln t read from A.lnt (b2n_integrate_lnt); the full h / logzvar arrays are written only in that mode, so the
+// instantiations of b2n_jitter_runs compile to the code they had before it existed.
+template <int PASS, bool GIVEN>
 __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     __shared__ double lt[JT_TILE], pv[JT_TILE], cap[JT_TILE + 1], buf[JT_CHUNK], wsum[32];
     const int64_t sg = blockIdx.x;
@@ -143,7 +157,7 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     const JSeg s = A.seg[sg];
     const int L = s.len;
     const int64_t so = (int64_t)r * A.nseg + sg;
-    segment_lnt(A, s, r, lt, cap, buf, wsum);
+    segment_lnt<GIVEN>(A, s, r, lt, cap, buf, wsum);
     for (int i = threadIdx.x; i < L; i += blockDim.x) pv[i] = lt[i];
     __syncthreads();
     const double D = block_scan(pv, L, wsum, OpSum());      // pv[i] = sum of lt[0..i]
@@ -189,7 +203,7 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
         const double dh = a - zmax * (exp(buf[i] - zmax) - exp((i > 0 ? buf[i - 1] : Z) - zmax));
         sa[i] = a;
         c_r[u] = dh * -lt[i];
-        if (A.wref) {
+        if (!GIVEN && A.wref) {             // (no KL divergence against given ln t)
             const double lp1 = cap[i] - zmax;
             k_r[u] = exp(lp1) * (lp1 - (A.wref[j] - A.zref));
         }
@@ -212,12 +226,21 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     const double Ksum = block_scan(pv, L, wsum, OpSum());
     if (A.f_kld)
         for (int i = threadIdx.x; i < L; i += blockDim.x) A.f_kld[fo + i] = pv[i];
+    if (GIVEN) {
+        // segment-local parts: h = h1 - zmax exp(logz - zmax) with h1's local prefix in sa; logzvar's local prefix
+        // in lt (the offsets launch adds the prefixes of the segments before)
+        if (A.f_h)
+            for (int i = threadIdx.x; i < L; i += blockDim.x) A.f_h[fo + i] = sa[i] - zmax * exp(buf[i] - zmax);
+        if (A.f_logzvar)
+            for (int i = threadIdx.x; i < L; i += blockDim.x) A.f_logzvar[fo + i] = lt[i];
+    }
     if (threadIdx.x == 0) { A.sA[so] = Asum; A.sC[so] = Csum; A.sK[so] = Ksum; }
 }
 
 // One realisation per block: running scans over its segments in chunks of JT_TILE.
 // PASS 1: logvol (sV) and logz (sZ) before every segment, zend = logz[-1].
-// PASS 2: the summaries; the kld prefix before every segment into sK (in place) when the full kld array is wanted.
+// PASS 2: the summaries; the kld prefix before every segment into sK (in place) when the full kld array is wanted,
+// likewise the h1 prefix into sA and the logzvar prefix into sC when the full h / logzvar arrays are.
 template <int PASS>
 __global__ void __launch_bounds__(JT_BLOCK) jitter_scan_kernel(JArgs A) {
     __shared__ double x[JT_TILE], y[JT_TILE], z[JT_TILE], wsum[32];
@@ -255,6 +278,10 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_scan_kernel(JArgs A) {
             const double tk = block_scan(z, m, wsum, OpSum());
             if (A.f_kld)
                 for (int i = threadIdx.x; i < m; i += blockDim.x) A.sK[base + g0 + i] = i > 0 ? c2 + z[i - 1] : c2;
+            if (A.f_h)
+                for (int i = threadIdx.x; i < m; i += blockDim.x) A.sA[base + g0 + i] = i > 0 ? c0 + x[i - 1] : c0;
+            if (A.f_logzvar)
+                for (int i = threadIdx.x; i < m; i += blockDim.x) A.sC[base + g0 + i] = i > 0 ? c1 + y[i - 1] : c1;
             c0 += ta;
             c1 += tc;
             c2 += tk;
@@ -273,13 +300,55 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_scan_kernel(JArgs A) {
     }
 }
 
-__global__ void __launch_bounds__(JT_BLOCK) jitter_kld_offsets_kernel(JArgs A) {
+// The prefixes scan 2 left in sK / sA / sC added to the segment-local full kld / h / logzvar arrays.
+__global__ void __launch_bounds__(JT_BLOCK) jitter_offsets_kernel(JArgs A) {
     const int64_t sg = blockIdx.x;
     const int r = blockIdx.y;
     const JSeg s = A.seg[sg];
-    const double off = A.sK[(int64_t)r * A.nseg + sg];
-    double* f = A.f_kld + (size_t)r * A.N + s.a;
-    for (int i = threadIdx.x; i < s.len; i += blockDim.x) f[i] += off;
+    const int64_t so = (int64_t)r * A.nseg + sg;
+    const size_t fo = (size_t)r * A.N + s.a;
+    if (A.f_kld) {
+        const double off = A.sK[so];
+        for (int i = threadIdx.x; i < s.len; i += blockDim.x) A.f_kld[fo + i] += off;
+    }
+    if (A.f_h) {
+        const double off = A.sA[so];
+        for (int i = threadIdx.x; i < s.len; i += blockDim.x) A.f_h[fo + i] += off;
+    }
+    if (A.f_logzvar) {                      // logzvar = |cumsum(dh * dlogvol)|
+        const double off = A.sC[so];
+        for (int i = threadIdx.x; i < s.len; i += blockDim.x) A.f_logzvar[fo + i] = fabs(A.f_logzvar[fo + i] + off);
+    }
+}
+
+// The passes on the stream for a prepared JArgs (seg, nseg, N, R and the scratch pointers set).
+int jitter_launch(b2n_ctx* ctx, const JArgs& A, bool given) {
+    const dim3 grid((unsigned)A.nseg, (unsigned)A.R);
+    if (given) jitter_pass_kernel<1, true><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else jitter_pass_kernel<1, false><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    jitter_scan_kernel<1><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    if (given) jitter_pass_kernel<2, true><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else jitter_pass_kernel<2, false><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    jitter_scan_kernel<2><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    if (A.f_kld || A.f_h || A.f_logzvar) {
+        jitter_offsets_kernel<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+        B2N_LAUNCH_CHECK(ctx);
+    }
+    return B2N_OK;
+}
+
+// Per-(realisation, segment) scratch: 7 x R x nseg, + logz[-1] per realisation.
+int jitter_scratch(b2n_ctx* ctx, JArgs& A) {
+    const size_t rs = (size_t)A.R * A.nseg;
+    B2N_CUDA(ctx, ctx->scratch1.ensure((7 * rs + A.R) * sizeof(double)));
+    double* sp = ctx->scratch1.as<double>();
+    A.sD = sp; A.sE = sp + rs; A.sV = sp + 2 * rs; A.sZ = sp + 3 * rs;
+    A.sA = sp + 4 * rs; A.sC = sp + 5 * rs; A.sK = sp + 6 * rs; A.zend = sp + 7 * rs;
+    return B2N_OK;
 }
 
 // The segment table and the per-sample aux words (the stretch plan; depends on samples_n only).  O(N), one pass.
@@ -354,12 +423,7 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
     A.seg = (const JSeg*)p;
     A.N = N; A.nseg = nseg; A.R = R; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0;
-    // per-(realisation, segment) scratch: 7 x R x nseg, + logz[-1] per realisation
-    const size_t rs = (size_t)R * nseg;
-    B2N_CUDA(ctx, ctx->scratch1.ensure((7 * rs + R) * sizeof(double)));
-    double* sp = ctx->scratch1.as<double>();
-    A.sD = sp; A.sE = sp + rs; A.sV = sp + 2 * rs; A.sZ = sp + 3 * rs;
-    A.sA = sp + 4 * rs; A.sC = sp + 5 * rs; A.sK = sp + 6 * rs; A.zend = sp + 7 * rs;
+    B2N_TRY(jitter_scratch(ctx, A));
     void* d;
     double* const sum_user[4] = {logz, logzerr, h, kld};
     double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
@@ -377,22 +441,32 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     }
 
     B2N_TIME_BEGIN(ctx);
-    const dim3 grid((unsigned)nseg, (unsigned)R);
-    jitter_pass_kernel<1><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
-    jitter_scan_kernel<1><<<R, JT_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
-    jitter_pass_kernel<2><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
-    jitter_scan_kernel<2><<<R, JT_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
-    if (A.f_kld) {
-        jitter_kld_offsets_kernel<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-        B2N_LAUNCH_CHECK(ctx);
-    }
+    B2N_TRY(jitter_launch(ctx, A, false));
     B2N_TIME_END(ctx);
 
     for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
     for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, full_user[k], *full_dev[k], (size_t)R * N * sizeof(double)));
     return b2n_finish(ctx);
+}
+
+// compute_integrals (utils.py:1411-1467) of one record whose ln t per sample is given: logvol = cumsum(lnt), then the
+// quadrature of the passes above.  Every pointer is a device pointer; the outputs may be NULL.  last3 (3 doubles):
+// logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1].  Enqueues on the context's stream and does not synchronise; uses
+// ctx->scratch0 and ctx->scratch1.
+int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
+                      double* logwt, double* logz, double* logzvar, double* h) {
+    std::vector<JSeg> seg;
+    for (int64_t a = 0; a < N; a += JT_TILE) seg.push_back(JSeg{a, (int32_t)std::min<int64_t>(JT_TILE, N - a), 0, 0});
+    if ((int64_t)seg.size() > INT32_MAX) return B2N_ERR_ARG;
+    JArgs A;
+    memset(&A, 0, sizeof(A));
+    const void* p;
+    B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
+    A.seg = (const JSeg*)p;
+    A.logl = logl; A.lnt = lnt;
+    A.N = N; A.nseg = (int64_t)seg.size(); A.R = 1;
+    B2N_TRY(jitter_scratch(ctx, A));
+    if (last3) { A.out_logz = last3; A.out_logzerr = last3 + 1; A.out_h = last3 + 2; }
+    A.f_logvol = logvol; A.f_logwt = logwt; A.f_logz = logz; A.f_logzvar = logzvar; A.f_h = h;
+    return jitter_launch(ctx, A, true);
 }

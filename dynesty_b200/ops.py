@@ -569,3 +569,46 @@ def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, cha
     if multiplicities:
         o['mult'] = m.astype(np.int64)
     return o
+
+
+def merge_runs(logl, samples_n, run_ptr, nbase, lowedge=None, arrays=True, ctx=None):
+    """R records merged into one (merge_runs / _merge_two, utils.py:1817-1900, 2045-2225; include/b200nest.h,
+    b2n_merge_runs).  logl / samples_n: the records concatenated, run r = [run_ptr[r], run_ptr[r + 1]), each run's
+    logl ascending; the first nbase runs are the base group (pairwise tree), the others add-on runs merged in order;
+    lowedge (R): each run's low edge (None: -inf for all).  Returns dict(perm, samples_n, logz_end, logzerr_end, h_end):
+    the index in the concatenation of every merged sample, the merged live counts and the last elements of logz,
+    logzerr and information; with arrays=True also logvol, logwt, logz, logzvar, h (N each)."""
+    logl = f64(logl)
+    n = np.ascontiguousarray(samples_n, dtype=np.int64)
+    rp = np.ascontiguousarray(run_ptr, dtype=np.int64)
+    N, R = len(logl), len(rp) - 1
+    if len(n) != N:
+        raise ValueError("logl and samples_n differ in length")
+    if R < 1 or rp[0] != 0 or rp[-1] != N or np.any(np.diff(rp) < 1):
+        raise ValueError("run_ptr must run from 0 to len(logl) through non-empty runs")
+    if not 1 <= int(nbase) <= R:
+        raise ValueError("nbase must lie in 1..%d" % R)
+    if np.isnan(logl).any():
+        raise ValueError("logl holds NaN")
+    inner = np.ones(max(N - 1, 0), dtype=bool)
+    inner[rp[1:-1] - 1] = False                   # pairs that straddle two runs
+    if np.any(np.diff(logl)[inner] < 0):
+        raise ValueError("the logl of every run must be ascending")
+    if np.any(n < 1):
+        raise ValueError("samples_n must be >= 1")
+    le = None
+    if lowedge is not None:
+        le = f64(lowedge)
+        if len(le) != R or np.isnan(le).any():
+            raise ValueError("lowedge must hold one number per run")
+    o = dict(perm=np.empty(N, dtype=np.int64), samples_n=np.empty(N, dtype=np.int64))
+    last = np.empty(3)
+    if arrays:
+        for k in ('logvol', 'logwt', 'logz', 'logzvar', 'h'):
+            o[k] = np.empty(N)
+    ctx = _ctx(ctx)
+    ctx.check(ctx.lib.b2n_merge_runs(ctx.h, ptr(logl), ptr(n), ptr(rp), R, int(nbase), ptr(le), ptr(o['perm']),
+                                     ptr(o['samples_n']), ptr(last), ptr(o.get('logvol')), ptr(o.get('logwt')),
+                                     ptr(o.get('logz')), ptr(o.get('logzvar')), ptr(o.get('h'))))
+    o.update(logz_end=float(last[0]), logzerr_end=float(last[1]), h_end=float(last[2]))
+    return o

@@ -5,6 +5,7 @@ What is mirrored (reference py/dynesty/utils.py, same names / meaning):
   resample_run  :1495-1660   one bootstrap realisation of a run's strands (the points that occupied one live slot)
   unravel_run   :1711-1814   a run split into its strands
   kld_error     :1932-1997   the KL divergence from the run to such a realisation
+  merge_runs    :1817-1929   several runs merged into one (``b2n_merge_runs``)
 and the batched forms the dynamic sampler's stopping function needs: ``jitter_realisations`` (``b2n_jitter_runs``) and
 ``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches.
 
@@ -236,3 +237,126 @@ def unravel_run(res):
             r['batch_bounds'] = res['batch_bounds']
         out.append(r)
     return out
+
+
+# ---------------------------------------------------------------------------------------------- merging runs
+def _batches(res):
+    """(per-sample batch, batch bounds) of a record: its own, or batch 0 with bounds (-inf, inf) (utils.py:2027-2041)."""
+    if 'samples_batch' in res and 'batch_bounds' in res:
+        return (np.asarray(res['samples_batch'], dtype=np.int64),
+                np.array([tuple(b) for b in res['batch_bounds']], dtype=float).reshape(-1, 2))
+    return np.zeros(len(res['logl']), dtype=np.int64), np.array([[-np.inf, np.inf]])
+
+
+def merge_order(res_list):
+    """merge_runs' grouping (utils.py:1842-1856): (order, nbase) -- the base runs (a sample in batch 0, or no batches
+    at all) in their order, then the add-on runs in theirs; one base run and one add-on run are both merged as base
+    runs, in the given order."""
+    base = [i for i, r in enumerate(res_list) if 'samples_batch' not in r or np.any(np.asarray(r['samples_batch']) == 0)]
+    add = [i for i in range(len(res_list)) if i not in set(base)]
+    if not base:
+        raise ValueError("merge_runs needs at least one run started from the prior (a sample in batch 0)")
+    if len(base) == 1 and len(add) == 1:
+        return [0, 1], 2
+    return base + add, len(base)
+
+
+def _strands_resolve(res):
+    """True when the record's strand columns can be resolved inside it: it ends with its final live points and every
+    samples_it > 0 names an earlier sample of the record's own batch with a logl not above the point's (a strand
+    that unravel_run cut out of a larger record does not)."""
+    if 'samples_id' not in res or 'samples_it' not in res:
+        return False
+    if 'samples_batch' not in res and len(res['logl']) <= int(res['niter']):
+        return False
+    logl = np.asarray(res['logl'], dtype=float)
+    batch = _batches(res)[0]
+    it = np.asarray(res['samples_it'], dtype=np.int64)
+    later = np.nonzero(it > 0)[0]
+    cnt = np.bincount(batch, minlength=int(batch.max()) + 1)
+    k = it[later] - 1
+    if np.any(k >= cnt[batch[later]]):
+        return False
+    prev = np.argsort(batch, kind='stable')[(np.cumsum(cnt) - cnt)[batch[later]] + k]
+    return bool(np.all(prev < later) and np.all(logl[prev] <= logl[later]))
+
+
+def check_result_static(res):
+    """check_result_static (utils.py:1903-1929): a record whose counts are those of a static run -- constant, or
+    constant with the final N, N-1, .., 1 tail -- gets nlive = that count and niter = its length - nlive."""
+    n = samples_n_of(res)
+    nlive, niter = int(n.max()), int(res['niter'])
+    if n.size == niter and (np.all(n == nlive) or np.all(n == np.minimum(np.arange(niter, 0, -1), nlive))):
+        res['nlive'], res['niter'] = nlive, niter - nlive
+    return res
+
+
+def merge_runs(res_list, ctx=None):
+    """merge_runs (utils.py:1817-1929): the runs of `res_list` merged into one run, e.g. an ensemble of replicas
+    into a run with the sum of their live points.  Base runs (started from the prior) merge as a pairwise tree,
+    add-on runs (a dynamic batch's strands, as unravel_run makes them) merge onto the result one at a time; the
+    order, the live counts, ln X (with the reference's plateau rule for equal logl) and the integrals are computed by
+    ``b2n_merge_runs``.  Positions (samples_u / samples), ncall_per_it and samples_scale are gathered here, and only
+    when every run carries them (a run made with keep_samples=False: empty positions); ncall is the sum.
+
+    Deliberate differences from the reference:
+      * samples_id is offset per run, so that the strands of different runs stay distinct (the reference keeps
+        the ids, and strand 0 of two static runs would collide);
+      * every (run, batch) pair is a batch of its own, with its bounds in batch_bounds (the reference merges equal
+        bounds, which would make samples_it meaningless across runs);
+      * samples_id / samples_it are kept only when every run carries them, ends with its final live points and
+        resolves them inside itself (see ``strand_plan``); otherwise they are dropped and resample_run raises
+        NotImplementedError on the merged run.
+    A single run is returned as it is (after check_result_static), as the reference does."""
+    res_list = list(res_list)
+    order, nbase = merge_order(res_list)
+    ndims = {np.shape(r[k])[1] for r in res_list for k in ('samples_u', 'samples') if k in r and np.ndim(r[k]) == 2}
+    if len(ndims) > 1:
+        raise ValueError("merge_runs: the runs differ in ndim (%s)" % sorted(ndims))
+    if len(res_list) == 1:
+        return check_result_static(Results(res_list[0]))
+    runs = [res_list[i] for i in order]
+    sizes = np.array([len(r['logl']) for r in runs], dtype=np.int64)
+    run_ptr = np.r_[0, np.cumsum(sizes)]
+    logl = np.concatenate([np.asarray(r['logl'], dtype=float) for r in runs])
+    lowedge = []
+    for r in runs:
+        b, bounds = _batches(r)
+        lowedge.append(float(np.min(bounds[b])))
+    o = ops.merge_runs(logl, np.concatenate([samples_n_of(r) for r in runs]), run_ptr, nbase, lowedge, arrays=True,
+                       ctx=ctx)
+    perm = o['perm']
+    N = len(perm)
+    ncall = int(sum(int(r['ncall']) if 'ncall' in r else int(np.sum(r['ncall_per_it'])) for r in runs))
+    new = Results(niter=N, ncall=ncall, eff=100. * N / max(ncall, 1), logl=logl[perm], samples_n=o['samples_n'],
+                  logvol=o['logvol'], logwt=o['logwt'], logz=o['logz'],
+                  logzerr=np.sqrt(np.maximum(o['logzvar'], 0)), information=o['h'])
+
+    def gather(k):
+        return np.concatenate([np.asarray(r[k]) for r in runs])[perm]
+
+    def complete(k):
+        return all(k in r and len(r[k]) == len(r['logl']) for r in runs)
+
+    for k in ('ncall_per_it', 'samples_scale'):
+        if complete(k):
+            new[k] = gather(k)
+    if ndims:
+        ndim = ndims.pop()
+        for k in ('samples_u', 'samples'):
+            new[k] = gather(k) if complete(k) else np.empty((0, ndim))
+    batch, bounds, boff = [], [], 0
+    for r in runs:
+        b, bd = _batches(r)
+        batch.append(b + boff)
+        bounds.extend(tuple(float(x) for x in row) for row in bd)
+        boff += len(bd)
+    new.update(samples_batch=np.concatenate(batch)[perm], batch_bounds=bounds)
+    if all(_strands_resolve(r) for r in runs):
+        ids, off = [], 0
+        for r in runs:
+            i = np.asarray(r['samples_id'], dtype=np.int64)
+            ids.append(i + off)
+            off += int(i.max()) + 1
+        new.update(samples_id=np.concatenate(ids)[perm], samples_it=gather('samples_it').astype(np.int64))
+    return check_result_static(new)

@@ -347,6 +347,31 @@ int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, i
                       const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
                       double* logz, double* logzerr, double* h, double* kld, int32_t* mult);
 
+/* ---- merge_runs (utils.py:1817-1900, _merge_two :2045-2225 of the reference) ---------------------------------------
+ * R dead-point records of N samples in all, concatenated: run r is samples [run_ptr[r], run_ptr[r + 1]), its logl
+ * ascending and free of NaN (assumed, not checked), samples_n its live count at every sample (>= 1).  The first nbase
+ * runs are the BASE group, merged as the reference's pairwise tree: (0, 1), (2, 3), .. per level, an odd run passes to
+ * the next level.  Runs nbase..R-1 are ADD-ON runs, merged onto the result one at a time in that order.
+ * Each merge of two runs is _merge_two's walk: the base side's point goes first on a tie; the merged point's count is
+ * the sum of both runs' counts at their current points (an exhausted run: logl +inf, count 0), except that only the
+ * base's count applies while the base's current logl <= the new run's low edge, and otherwise only the new run's while
+ * the new run's current logl <= the base's low edge.  lowedge[r]: run r's low edge, the least lower bound of the
+ * batches its samples belong to (-inf for a run started from the prior; NULL: -inf for every run); a merged run's is
+ * the lesser of its two.
+ * Then ln X (:2159-2187): ln t = ln(n / (n + 1)) per merged sample, except inside a group of m >= 2 equal logl whose
+ * first point has count n, where the k-th point (k = 0..m-1) gets ln((n - k) / (n - k + 1)) (a group longer than n + 1
+ * gives non-finite volumes); logvol = cumsum(ln t), and the trapezoid integrals of compute_integrals (:1411-1467).
+ * run_ptr (R + 1, run_ptr[0] = 0, every run non-empty) and lowedge (R): HOST.  logl, samples_n (int64): N.
+ * Outputs, each may be NULL: perm (N, int64): the index in the concatenation of every merged sample; samples_n_out
+ * (N, int64): the merged counts; last3 (3): logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1]; logvol, logwt, logz,
+ * logzvar, h (N each): the full arrays of compute_integrals.
+ * FP64 / int64, no atomics: the outputs are the same bits from call to call.  1 + ceil(log2 nbase) + (R - nbase) + 1
+ * merge launches, then the 4 or 5 of the quadrature, with no host round trip.  1 <= nbase <= R <= 2^31 - 1, N >= 1.
+ * Synchronises in host-pointer mode. */
+int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, const int64_t* run_ptr, int32_t R,
+                   int32_t nbase, const double* lowedge, int64_t* perm, int64_t* samples_n_out, double* last3,
+                   double* logvol, double* logwt, double* logz, double* logzvar, double* h);
+
 /* ---- resident bound for the proposal kernels --------------------------------
  * Uploads K ellipsoids of dimension ncdim (what Sampler ships to every task as
  * `axes` / kwargs['bound'], sampler.py:708-717, internal_samplers.py:229-233).
