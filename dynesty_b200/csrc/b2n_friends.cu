@@ -282,9 +282,15 @@ int b2n_friends_update(b2n_ctx* ctx, const double* points, int64_t N, int32_t n,
     if (!ctx || !points || N < 2 || n < 1 || (kind != 0 && kind != 1) || nboot < 0) return B2N_ERR_ARG;
     if (use_clustering && !am_prev) return B2N_ERR_ARG;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int ld = n | 1, half = ((n + 1) & ~1) >> 1;
-    const size_t met_smem = (size_t)(2 * half + 4 * n + 32 + 2 * n * ld) * sizeof(double);
-    if (met_smem > (size_t)ctx->max_smem_optin) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the friends bounds (n <= ~117)");
+    const int ld = n | 1;
+    auto metric_smem = [](int m) { return (size_t)(2 * (((m + 1) & ~1) >> 1) + 4 * m + 32 + 2 * m * (m | 1)) * sizeof(double); };
+    const size_t met_smem = metric_smem(n);
+    if (met_smem > (size_t)ctx->max_smem_optin) {
+        int nmax = n;
+        while (nmax > 1 && metric_smem(nmax) > (size_t)ctx->max_smem_optin) nmax--;
+        snprintf(ctx->err, sizeof(ctx->err), "ndim %d too large for the friends bounds (n <= %d on this device)", n, nmax);
+        return B2N_ERR_UNSUPPORTED;
+    }
     if (N > (1 << 20)) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "too many points for the friends bounds");
     cudaStream_t st = ctx->stream;
     const size_t nn = (size_t)n * n;
