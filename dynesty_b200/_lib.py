@@ -86,6 +86,7 @@ SYMBOLS = {
     'b2n_membership': (C.c_int, [_P, _P, _L, _I, _P, _P, _I, _I, _P, _P, _P]),
     'b2n_bounding_ellipsoid': (C.c_int, [_P, _P, _L, _I, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_multi_decompose': (C.c_int, [_P, _P, _L, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'b2n_multi_tree': (C.c_int, [_P, _P, _L, _I, _I, _P, _P, _P, _P, _P]),
     'b2n_moments': (C.c_int, [_P, _P, _L, _I, _P, _P]),
     'b2n_improve_covar': (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P]),
     'b2n_fp64_peak': (C.c_int, [_P, _I, _I, C.POINTER(_D), C.POINTER(_D)]),

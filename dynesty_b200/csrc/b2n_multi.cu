@@ -293,6 +293,7 @@ __global__ void scatter_labels_kernel(const int* __restrict__ perm, int start, i
 struct HNode {
     int start, count, level;
     int child[2];
+    int split[2];         // the two cluster sizes of the node's k-means split, -1 if none was attempted
     double logvol;
 };
 
@@ -340,7 +341,7 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
     cudaStream_t st = ctx->stream;
     tree.clear();
     HNode root;
-    root.start = 0; root.count = count; root.level = 0; root.child[0] = root.child[1] = -1; root.logvol = 0;
+    root.start = 0; root.count = count; root.level = 0; root.child[0] = root.child[1] = -1; root.split[0] = root.split[1] = -1; root.logvol = 0;
     tree.push_back(root);
     std::vector<NodeRef> refs(1);
     memset(&refs[0], 0, sizeof(NodeRef));
@@ -440,14 +441,15 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
         std::vector<NodeRef> crefs;
         for (size_t i = 0; i < split.size(); i++) {
             const int c0 = hc[2 * i], c1 = hc[2 * i + 1];
-            if (std::min(c0, c1) < min_size) continue;                    // :1521-1522
             const int id = split[i];
+            tree[id].split[0] = c0; tree[id].split[1] = c1;
+            if (std::min(c0, c1) < min_size) continue;                    // :1521-1522
             if ((int)tree.size() + 2 > w.cap) return b2n_fail(ctx, B2N_ERR_TOO_MANY_ELLS, "node capacity exceeded");
             for (int k = 0; k < 2; k++) {
                 HNode ch;
                 ch.start = tree[id].start + (k ? c0 : 0);
                 ch.count = k ? c1 : c0;
-                ch.level = cur; ch.child[0] = ch.child[1] = -1; ch.logvol = 0;
+                ch.level = cur; ch.child[0] = ch.child[1] = -1; ch.split[0] = ch.split[1] = -1; ch.logvol = 0;
                 tree[id].child[k] = (int)tree.size();
                 NodeRef r;
                 memset(&r, 0, sizeof(r));
@@ -522,22 +524,18 @@ static int gather_leaves(BoundWork& w, const std::vector<int>& leaves, double** 
     return B2N_OK;
 }
 
-extern "C" int b2n_multi_decompose(b2n_ctx* ctx, const double* points, int64_t N, int32_t n, int32_t max_ells,
-                                   int32_t* nells, int32_t* labels, double* ctrs, double* covs, double* ams,
-                                   double* axes, double* axlens, double* logvols, uint32_t* warn) {
-    if (!ctx || !points || N < 1 || n < 1 || max_ells < 1 || !nells) return B2N_ERR_ARG;
-    if (N == 1) return B2N_ERR_SINGLE_POINT;
+// The decomposition of b2n_multi_decompose and b2n_multi_tree: the points uploaded, the candidate path chosen, the
+// tree expanded and resolved, and redone with the eigen path if a candidate could not be certified.  *fast_used:
+// the tree returned is the one of the Cholesky candidates.
+static int multi_run(b2n_ctx* ctx, const double* points, int64_t N, int n, BoundWork& w, const void** dP,
+                     std::vector<HNode>& tree, std::vector<int>& leaves, int& level, uint32_t* warn, bool* fast_used) {
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     if (warn) *warn = 0;
-    const void* dP;
-    B2N_TRY(b2n_in(ctx, ctx->in0, points, (size_t)N * n * sizeof(double), &dP));
-    BoundWork w;
+    B2N_TRY(b2n_in(ctx, ctx->in0, points, (size_t)N * n * sizeof(double), dP));
     const int cap = (int)std::max<int64_t>(3, N / std::max(n, 1) + 3);
-    B2N_TRY(b2n_boundwork_init(ctx, w, (const double*)dP, N, n, cap));
+    B2N_TRY(b2n_boundwork_init(ctx, w, (const double*)*dP, N, n, cap));
     B2N_TRY(b2n_init_identity_perm(w));
-    std::vector<HNode> tree;
-    std::vector<int> leaves;
-    int level = 0;
+    level = 0;
     // candidates through the Cholesky path when the two work matrices fit in shared memory (n <= ~117)
     // and the path has not just failed to certify a node of this problem (ctx->bound_fast_skip)
     const char* fenv = getenv("B2N_BOUND_FAST");
@@ -545,13 +543,30 @@ extern "C" int b2n_multi_decompose(b2n_ctx* ctx, const double* points, int64_t N
     bool fast = !(fenv && !strcmp(fenv, "0")) && N >= 4 * (int64_t)n &&
                 (size_t)(2 * n * ldw + 3 * n + 32 + 2 * (n + 2)) * sizeof(double) <= (size_t)ctx->max_smem_optin;
     if (fast && ctx->bound_fast_skip > 0 && !(fenv && fenv[0] == '1')) { ctx->bound_fast_skip--; fast = false; }   // "1" forces the attempt
+    *fast_used = fast;
     int dst = decompose(w, (int)N, tree, leaves, level, warn, fast);
     if (dst == B2N_RETRY_FULL) {
         ctx->bound_fast_skip = 16;
+        *fast_used = false;
         if (warn) *warn = 0;
         B2N_TRY(b2n_init_identity_perm(w));
         dst = decompose(w, (int)N, tree, leaves, level, warn, false);
     }
+    return dst;
+}
+
+extern "C" int b2n_multi_decompose(b2n_ctx* ctx, const double* points, int64_t N, int32_t n, int32_t max_ells,
+                                   int32_t* nells, int32_t* labels, double* ctrs, double* covs, double* ams,
+                                   double* axes, double* axlens, double* logvols, uint32_t* warn) {
+    if (!ctx || !points || N < 1 || n < 1 || max_ells < 1 || !nells) return B2N_ERR_ARG;
+    if (N == 1) return B2N_ERR_SINGLE_POINT;
+    const void* dP;
+    BoundWork w;
+    std::vector<HNode> tree;
+    std::vector<int> leaves;
+    int level = 0;
+    bool fast_used = false;
+    const int dst = multi_run(ctx, points, N, n, w, &dP, tree, leaves, level, warn, &fast_used);
     if (dst != B2N_OK) return dst;
     const int K = (int)leaves.size();
     *nells = K;
@@ -591,6 +606,35 @@ extern "C" int b2n_multi_decompose(b2n_ctx* ctx, const double* points, int64_t N
         B2N_TRY(b2n_out_done(ctx, labels, dl, (size_t)N * sizeof(int)));
     }
     B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return B2N_OK;
+}
+
+extern "C" int b2n_multi_tree(b2n_ctx* ctx, const double* points, int64_t N, int32_t n, int32_t max_nodes,
+                              int32_t* nnodes, int32_t* nodes, double* logvols, int32_t* perm, int32_t* path) {
+    if (!ctx || !points || N < 1 || n < 1 || max_nodes < 1 || !nnodes || !nodes || !logvols || !perm || !path)
+        return B2N_ERR_ARG;
+    if (N == 1) return B2N_ERR_SINGLE_POINT;
+    const void* dP;
+    BoundWork w;
+    std::vector<HNode> tree;
+    std::vector<int> leaves;
+    int level = 0;
+    bool fast_used = false;
+    B2N_TRY(multi_run(ctx, points, N, n, w, &dP, tree, leaves, level, nullptr, &fast_used));
+    const int T = (int)tree.size();
+    *nnodes = T;
+    if (T > max_nodes) return B2N_ERR_TOO_MANY_ELLS;
+    std::vector<int> accepted(T, 0);
+    for (int id : leaves) accepted[id] = 1;
+    for (int i = 0; i < T; i++) {
+        const HNode& nd = tree[i];
+        const int row[7] = {nd.start, nd.count, nd.child[0], nd.child[1], nd.split[0], nd.split[1], accepted[i]};
+        memcpy(nodes + (size_t)7 * i, row, sizeof(row));
+        logvols[i] = nd.logvol;
+    }
+    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    B2N_CUDA(ctx, b2n_copy_sync(ctx, perm, w.perm + (size_t)level * N, (size_t)N * sizeof(int), cudaMemcpyDeviceToHost));
+    *path = fast_used ? 1 : 0;
     return B2N_OK;
 }
 

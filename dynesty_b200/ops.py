@@ -82,6 +82,26 @@ def multi_decompose(points, max_ells=None, ctx=None):
     return o
 
 
+def multi_tree(points, ctx=None):
+    """Diagnostic: the candidate tree b2n_multi_decompose builds on `points`.  dict(start, count, children (T, 2),
+    split (T, 2), logvol, leaf (bool), perm (N,), path 'cholesky' | 'eigen'); node i's points are
+    perm[start[i]:start[i] + count[i]] as a set, -1 marks no child / no split attempted."""
+    ctx = _ctx(ctx)
+    points = f64(points)
+    N, n = points.shape
+    cap = max(3, N // n + 3)
+    nodes = np.empty((cap, 7), dtype=np.int32)
+    logvols = np.empty(cap)
+    perm = np.empty(N, dtype=np.int32)
+    T, path = C.c_int32(0), C.c_int32(0)
+    ctx.check(ctx.lib.b2n_multi_tree(ctx.h, ptr(points), N, n, cap, C.addressof(T), ptr(nodes), ptr(logvols),
+                                     ptr(perm), C.addressof(path)))
+    t = nodes[:T.value]
+    return dict(start=t[:, 0].copy(), count=t[:, 1].copy(), children=t[:, 2:4].copy(), split=t[:, 4:6].copy(),
+                leaf=t[:, 6] == 1, logvol=logvols[:T.value].copy(), perm=perm,
+                path='cholesky' if path.value else 'eigen')
+
+
 def moments(points, ctx=None):
     """(mean, cov) = (np.mean(points, 0), np.cov(points, rowvar=False)) of one shard of the live set."""
     ctx = _ctx(ctx)

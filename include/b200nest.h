@@ -258,6 +258,21 @@ int b2n_multi_decompose(b2n_ctx* ctx, const double* points, int64_t N, int32_t n
                         double* ctrs, double* covs, double* ams, double* axes,
                         double* axlens, double* logvols, uint32_t* warn);
 
+/* DIAGNOSTIC, not on the sampling path: the candidate tree of b2n_multi_decompose.  Runs exactly the
+ * decomposition b2n_multi_decompose runs on the same points -- the same choice of the Cholesky candidate
+ * path (B2N_BOUND_FAST, the context's skip count after a failed certification) and the same redo with the
+ * eigen path -- and returns the tree instead of the leaves.  *nnodes (host int): nodes in the tree; the call
+ * fails with B2N_ERR_TOO_MANY_ELLS if that exceeds max_nodes (N / n + 3 always suffices).  Node i (node 0
+ * is the root; children follow their parent) fills nodes[7 i .. 7 i + 6] = { start, count, child 0, child 1
+ * (-1: none), the two cluster sizes of its 2-means split (-1: no split attempted; a split refused by the 2n
+ * minimum has sizes but no children), 1 if it is an accepted leaf } and logvols[i] = its log-volume: the
+ * candidate fit's, or the final eigen fit's for an accepted leaf.  The node's points are the rows
+ * perm[start .. start + count) as a SET (perm[N]: the row order the last partition left).  *path = 1 if the
+ * tree came from the Cholesky candidates, 0 from the eigen path.  nodes, logvols, perm and path are host
+ * arrays in either pointer mode.  Synchronises. */
+int b2n_multi_tree(b2n_ctx* ctx, const double* points, int64_t N, int32_t n, int32_t max_nodes,
+                   int32_t* nnodes, int32_t* nodes, double* logvols, int32_t* perm, int32_t* path);
+
 /* Block moments for a row-SHARDED live set (SURVEY.md 8e): mean (n) and sample covariance (n x n, ddof = 1; zeros
  * for a single row) of `points` (N x n) -- np.mean / np.cov of bounding.py:1410-1412 for one shard.  Shards combine
  * exactly: S = sum_r [(N_r - 1) cov_r + N_r (mean_r - mean)(mean_r - mean)^T], cov = S / (N - 1); the ellipsoid then

@@ -261,3 +261,99 @@ def bootstrap_expand(points, sel_in, multi):
         ells, _ = bounding_ellipsoids(pin, ell)
         d = np.min(np.array([np.sqrt(e.mahal2(pout)) for e in ells]), axis=0)
     return max(1., float(np.max(d)))
+
+
+# ---- the whole candidate tree of bounding_ellipsoids, with what makes a comparison with it well-posed
+def kmeans2_trace(data, centres, niter=10):
+    """kmeans2_matrix with its conditioning: (labels, margin, late) where margin is the smallest relative
+    distance gap |d0 - d1| / (d0 + d1) of any point in any of the niter assignments (two centres) and late
+    says whether the last assignment changed any label of the one before."""
+    code = np.array(centres, dtype=float)
+    margin, prev, late = np.inf, None, False
+    for _ in range(niter):
+        d2 = ((data[:, None, :] - code[None, :, :])**2).sum(axis=2)
+        label = np.argmin(d2, axis=1)
+        s = d2[:, 0] + d2[:, 1]
+        gap = np.abs(d2[:, 0] - d2[:, 1])
+        margin = min(margin, float(np.min(np.where(s > 0, gap / np.where(s > 0, s, 1.0), 0.0))))
+        late = prev is not None and bool(np.any(label != prev))
+        prev = label
+        for j in range(2):
+            m = label == j
+            if m.any():
+                code[j] = data[m].mean(axis=0)
+    return prev, margin, late
+
+
+def candidate_tree(points, nparam=None):
+    """bounding_ellipsoids restated to return the WHOLE candidate tree (the reference fits both children of every
+    split before it applies its volume tests, :1525-1560, so the tree does not depend on the tests).
+
+    Returns dict(nodes, leaves, km_margin, eig_gap, late).  nodes[i]: members (sorted indices into `points`),
+    ell (its bounding_ellipsoid), logvol, depth, children (two node ids or None), split (the k-means cluster sizes,
+    None if no split was attempted), accept (None: no children; 0 rejected, 1 accepted by the first volume test
+    :1552, 2 by the second :1558) and dist (how far the evaluated tests lie from their thresholds, in ln volume).
+    leaves: the accepted leaves in the reference's order.  km_margin: smallest relative k-means margin over every
+    split node, point and Lloyd iteration; eig_gap: smallest relative gap between the two largest eigenvalues of a
+    split node's covariance (it fixes the major axis and so the start centres); late: some split node's labels
+    still changed in the last Lloyd iteration.  nparam overrides n (n + 3) / 2 (:1541)."""
+    points = np.asarray(points, dtype=float)
+    npts, n = points.shape
+    min_size = 2 * n
+    scale = points.std(axis=0)[None, :]
+    if nparam is None:
+        nparam = (n * (n + 3)) // 2
+    nodes = []
+    cond = dict(km_margin=np.inf, eig_gap=np.inf, late=False)
+
+    def expand(idx, ell, depth):
+        i = len(nodes)
+        nodes.append(dict(members=idx, ell=ell, logvol=ell.logvol, depth=depth, children=None, split=None,
+                          accept=None, dist=()))
+        if len(idx) < 2 * min_size:                               # :1493
+            return i
+        lam = np.sort(ell.axlens)**2
+        if n > 1:
+            cond['eig_gap'] = min(cond['eig_gap'], (lam[-1] - lam[-2]) / lam[-1])
+        p1, p2 = ell.major_axis_endpoints()
+        labels, margin, late = kmeans2_trace(points[idx] / scale, np.vstack((p1, p2)) / scale)
+        cond['km_margin'] = min(cond['km_margin'], margin)
+        cond['late'] = cond['late'] or late
+        sel = [labels == 0, labels == 1]
+        nodes[i]['split'] = (int(sel[0].sum()), int(sel[1].sum()))
+        if min(nodes[i]['split']) < min_size:                      # :1521
+            return i
+        nodes[i]['children'] = [expand(idx[s], bounding_ellipsoid(points[idx[s]]), depth + 1) for s in sel]
+        return i
+
+    def resolve(i):
+        nd = nodes[i]
+        if nd['children'] is None:
+            return [i]
+        c0, c1 = nd['children']
+        sub = resolve(c0) + resolve(c1)
+        cnt = len(nd['members'])
+        dec = nparam * math.log(cnt) / cnt                       # :1541-1542
+        t1 = np.logaddexp(nodes[c0]['logvol'], nodes[c1]['logvol']) - nd['logvol'] + dec
+        t2 = logsumexp([nodes[s]['logvol'] for s in sub]) - nd['logvol'] + dec * (len(sub) - 1)
+        if t1 < 0:
+            nd['accept'], nd['dist'] = 1, (abs(t1),)
+            return sub
+        nd['dist'] = (abs(t1), abs(t2))
+        nd['accept'] = 2 if t2 < 0 else 0
+        return sub if t2 < 0 else [i]
+
+    expand(np.arange(npts), bounding_ellipsoid(points), 0)
+    leaves = resolve(0)
+    return dict(nodes=nodes, leaves=leaves, **cond)
+
+
+def decision_margin(tree):
+    """Smallest distance of an evaluated volume test from its threshold (inf if nothing was split)."""
+    return min([d for nd in tree['nodes'] for d in nd['dist']], default=np.inf)
+
+
+def tree_by_members(tree):
+    """{tuple(sorted members): node id}: children are matched by their member SETS, because the sign of the
+    major-axis eigenvector (LAPACK's or the CUDA solver's) decides which end point seeds cluster 0."""
+    return {tuple(nd['members']): i for i, nd in enumerate(tree['nodes'])}

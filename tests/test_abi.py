@@ -30,7 +30,7 @@ def lib():
 
 def test_header_declares_the_path():
     d = _declared()
-    for must in ('b2n_init', 'b2n_bounding_ellipsoid', 'b2n_multi_decompose', 'b2n_membership',
+    for must in ('b2n_init', 'b2n_bounding_ellipsoid', 'b2n_multi_decompose', 'b2n_multi_tree', 'b2n_membership',
                  'b2n_scale_to_logvol', 'b2n_bootstrap_expand', 'b2n_bound_set', 'b2n_rwalk_batch',
                  'b2n_rslice_batch', 'b2n_slice_batch', 'b2n_unif_batch', 'b2n_peer_export', 'b2n_peer_import'):
         assert must in d
