@@ -22,6 +22,16 @@ WARN_IDENTITY_FALLBACK, WARN_DOUBLING, WARN_Q0_SLACK, WARN_UNIF_INEFFICIENT = 1,
  ERR_Q0, ERR_SLICE_FAIL, ERR_NOMEM, ERR_UNSUPPORTED, ERR_TOO_MANY_ELLS, ERR_PEER, ERR_PLATEAU) = range(14)
 PEER_HANDLE_BYTES, MAX_PEERS = 64, 8
 
+# The outputs of the chain samplers after u, v and logl, by slot of the exchange window (include/b200nest.h): three
+# int32 counters, then the uint32 flags; None = a slot the sampler does not return.  In argument order of the
+# b2n_*_batch entry points.
+CHAIN_OUTPUTS = {
+    'rwalk': ('n_accept', 'n_reject', 'ncall', None),
+    'slice': ('n_expand', 'n_contract', 'ncall', 'flags'),
+    'unif': ('ncall', 'nprop', None, 'flags'),
+    'unitcube': ('ncall', None, None, None),
+}
+
 
 class B200Unavailable(RuntimeError):
     """libb200nest.so / a CUDA device is missing.  The B200 path has no CPU fallback."""
@@ -282,8 +292,8 @@ class Context:
         return a
 
     def peer_gathered(self, total_rows, ndim, names):
-        """The complete outputs of the last gather-mode call, read from the own window:
-        u, v, logl and the call's int32 outputs under `names` (argument order, None = skip)."""
+        """The complete outputs of the last gather-mode call, read from the own window: u, v, logl and the slots after
+        them under `names` (window slot order, None = skip; CHAIN_OUTPUTS[sampler] names all of a sampler's)."""
         _, off = self.peer_result()
         o = dict(u=self.peer_read(off[0], (total_rows, ndim), np.float64),
                  v=self.peer_read(off[1], (total_rows, ndim), np.float64),

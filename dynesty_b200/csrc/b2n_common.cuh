@@ -173,14 +173,36 @@ int b2n_bound_set_dev(b2n_ctx* ctx, int K, int nc, const double* dctrs, const do
 int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
                       double* logwt, double* logz, double* logzvar, double* h);
 
-// gather-mode plumbing shared by the chain entry points (b2n_peer.cu).  b2n_peer_begin: when
-// gather mode is on, point the 7 output arrays at this rank's rows of its own window and fill
-// `ps`; returns through *on whether it did.  b2n_peer_end: copy the gathered arrays (total rows)
-// to the caller's pointers and fetch the error word; b2n_peer_finish replaces b2n_finish.
-int b2n_peer_begin(b2n_ctx* ctx, int n, PeerSet* ps, void** dev7, bool* on);
-int b2n_peer_end(b2n_ctx* ctx, int n, void* const* user7);
-int b2n_peer_finish(b2n_ctx* ctx, bool on);
 void b2n_peer_release(b2n_ctx* ctx);
+
+// ---- host side shared by the chain entry points (b2n_peer.cu) ----------------------------------------------------
+// A chain call's outputs, in the slot order of the exchange window: u, v (n f64 per row), logl (f64), three int32
+// counters, the uint32 flags.  An entry point passes them as `void* out[B2N_NSLOT]`, NULL for a slot it has not.
+enum { B2N_SLOT_FLAGS = 6, B2N_NSLOT = 7 };
+static inline uint64_t b2n_slot_row_bytes(int slot, int n) { return slot < 2 ? (uint64_t)n * 8 : (slot == 2 ? 8 : 4); }
+// Flag bit -> status of a call (msg NULL: the status alone).
+struct B2nFlagStatus {
+    uint32_t bit;
+    int status;
+    const char* msg;
+};
+// Checks every chain entry point starts with: ctx and args, then a pending b2n_set_start_rows (for the next
+// b2n_rwalk_batch only: refused and cleared, so that it never lingers), then the model (draw_only: a placeholder of
+// a->ndim dimensions that evaluates nothing).
+int b2n_chain_begin(b2n_ctx* ctx, const b2n_chain_args* a, bool draw_only, B2nModel* m);
+// Q == 0 after the entry point's own checks: nothing to do, except that in gather mode every rank must run a chain.
+int b2n_chain_none(b2n_ctx* ctx);
+// Device-paced launch (b2n_ns.cu): record the chains per CTA the entry point plans for; a launch (not a planning
+// pass) needs device pointers and no gather mode.
+int b2n_chain_dyn(b2n_ctx* ctx, int chains_per_cta);
+// dev[k]: where the kernel writes slot k -- this rank's rows of the exchange window in gather mode (*ps filled),
+// else out[k] itself or its staging buffer ctx->out<k> (b2n_out).
+int b2n_chain_bind(b2n_ctx* ctx, int n, int64_t Q, void* const* out, void** dev, PeerSet* ps);
+// The outputs back to the caller: all ranks' rows from the window in gather mode, else the staged ones.  With a
+// table of flag bits (ntab > 0) the flags of every row are summarised on the device first, the call synchronises, and
+// the first bit of the table that is set in any row gives the status.  A peer that never arrived is B2N_ERR_PEER.
+int b2n_chain_end(b2n_ctx* ctx, int n, int64_t Q, void* const* out, void* const* dev, const B2nFlagStatus* tab,
+                  int ntab);
 
 #define B2N_CUDA(ctx, call)                                                        \
     do {                                                                           \

@@ -485,23 +485,19 @@ int b2n_friends_overlap(b2n_ctx* ctx, const double* x, int64_t M, int32_t n, int
 
 int b2n_friends_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, double* v, double* logl, int32_t* ncall,
                            int32_t* nprop, uint32_t* flags) {
-    if (!ctx || !a || !u || !v || !logl || !ncall || !nprop || !flags) return B2N_ERR_ARG;
-    FriendsState* f = friends_of(ctx);
-    const int draw_only = (a->reserved & B2N_OPT_DRAW_ONLY) ? ((a->reserved & B2N_OPT_DRAW_MIXTURE) ? 3 : 1) : 0;
     B2nModel m;
-    memset(&m, 0, sizeof(m));
-    m.ndim = a->ndim;
-    m.like_kind = B2N_LIKE_EGGBOX;
-    if (!draw_only) {
-        if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-        m = ctx->models[a->model_id];
-    }
+    B2N_TRY(b2n_chain_begin(ctx, a, a && (a->reserved & B2N_OPT_DRAW_ONLY), &m));
+    const int draw_only = (a->reserved & B2N_OPT_DRAW_ONLY) ? ((a->reserved & B2N_OPT_DRAW_MIXTURE) ? 3 : 1) : 0;
+    if (!u || !v || !logl || !ncall || !nprop || !flags) return B2N_ERR_ARG;
+    if (ctx->peer.total > 0) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "friends sampling has no gather mode");
+    FriendsState* f = friends_of(ctx);
     const int n = a->ndim;
     const int64_t Q = a->nchain;
     if (f->N < 1 || f->n != n || n != m.ndim || a->ncdim != n || Q < 0)
         return b2n_fail(ctx, B2N_ERR_ARG, "friends sampling needs a resident friends bound with ncdim == ndim");
     if (Q == 0) return B2N_OK;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    ZcScope zc(ctx);          // pinned caller buffers are written in place (host-pointer mode)
     const void* dfl_in = nullptr;
     std::vector<uint32_t> fl;
     if (a->dimflags) {
@@ -512,14 +508,12 @@ int b2n_friends_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, dou
     p.m = m; p.n = n; p.N = f->N; p.kind = f->kind; p.draw_only = draw_only;
     p.ctrs = f->ctrs.as<double>(); p.ctrs_t = f->ctrs_t.as<double>(); p.axes = f->axes.as<double>(); p.axes_inv = f->axes_inv.as<double>();
     p.dimflags = (const uint32_t*)dfl_in; p.loglstar = a->loglstar; p.seed = a->seed; p.chain0 = a->chain0; p.Q = Q;
-    void *du, *dv, *dl, *dnc, *dnp, *dfl;
-    B2N_TRY(b2n_out(ctx, ctx->out0, u, (size_t)Q * n * sizeof(double), &du));
-    B2N_TRY(b2n_out(ctx, ctx->out1, v, (size_t)Q * n * sizeof(double), &dv));
-    B2N_TRY(b2n_out(ctx, ctx->out2, logl, (size_t)Q * sizeof(double), &dl));
-    B2N_TRY(b2n_out(ctx, ctx->out3, ncall, (size_t)Q * sizeof(int), &dnc));
-    B2N_TRY(b2n_out(ctx, ctx->out4, nprop, (size_t)Q * sizeof(int), &dnp));
-    B2N_TRY(b2n_out(ctx, ctx->out6, flags, (size_t)Q * sizeof(uint32_t), &dfl));
-    p.u = (double*)du; p.v = (double*)dv; p.logl = (double*)dl; p.ncall = (int*)dnc; p.nprop = (int*)dnp; p.flags = (uint32_t*)dfl;
+    void* const out[B2N_NSLOT] = {u, v, logl, ncall, nprop, nullptr, flags};
+    void* dev[B2N_NSLOT];
+    PeerSet none;
+    B2N_TRY(b2n_chain_bind(ctx, n, Q, out, dev, &none));
+    p.u = (double*)dev[0]; p.v = (double*)dev[1]; p.logl = (double*)dev[2]; p.ncall = (int*)dev[3]; p.nprop = (int*)dev[4];
+    p.flags = (uint32_t*)dev[6];
     const int threads = 128, wpb = threads / 32;
     const size_t smem = (size_t)wpb * 5 * n * sizeof(double);
     if (smem > (size_t)ctx->max_smem_optin) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the friends kernel");
@@ -536,13 +530,7 @@ int b2n_friends_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, dou
     }
 #undef CALL
     B2N_LAUNCH_CHECK(ctx);
-    B2N_TRY(b2n_out_done(ctx, u, du, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, v, dv, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, logl, dl, (size_t)Q * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, ncall, dnc, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, nprop, dnp, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, flags, dfl, (size_t)Q * sizeof(uint32_t)));
-    return b2n_finish(ctx);
+    return b2n_chain_end(ctx, n, Q, out, dev, nullptr, 0);
 }
 
 }  // extern "C"

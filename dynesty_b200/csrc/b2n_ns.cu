@@ -585,13 +585,11 @@ static int ns_chain_call(b2n_ctx* ctx, b2n_ns* ns, bool plan_only) {
     ctx->dyn.dev = d.dyn; ctx->dyn.order = d.order; ctx->dyn.cta = d.cta;
     ctx->dyn.max_cta = d.cpc > 0 ? d.K / d.cpc + d.Kell : 1;
     int st;
-    if (ns->phase == 0) {
-        if (plan_only) { ctx->dyn.cpc = 1; st = B2N_OK; }
-        else st = b2n_unitcube_batch(ctx, &a, d.o_u, d.o_v, d.o_logl, d.o_ncall, d.o_flags);
-    } else if (d.sampler == 3) {
-        if (plan_only) { ctx->dyn.cpc = 1; st = B2N_OK; }
-        else st = b2n_unif_batch(ctx, &a, d.o_u, d.o_v, d.o_logl, d.o_ncall, d.o_i0, d.o_flags);
-    } else if (d.sampler == 0)
+    if (ns->phase == 0)
+        st = b2n_unitcube_batch(ctx, &a, d.o_u, d.o_v, d.o_logl, d.o_ncall, d.o_flags);
+    else if (d.sampler == 3)
+        st = b2n_unif_batch(ctx, &a, d.o_u, d.o_v, d.o_logl, d.o_ncall, d.o_i0, d.o_flags);
+    else if (d.sampler == 0)
         st = b2n_rwalk_batch(ctx, &a, ns->cfg.steps, d.o_u, d.o_v, d.o_logl, d.o_i0, d.o_i1, d.o_ncall);
     else if (d.sampler == 1)
         st = b2n_rslice_batch(ctx, &a, ns->cfg.steps, 0, d.o_u, d.o_v, d.o_logl, d.o_i0, d.o_i1, d.o_ncall, d.o_flags);

@@ -15,15 +15,14 @@
 static inline uint64_t al256(uint64_t b) { return (b + 255) & ~(uint64_t)255; }
 
 static uint64_t slot_bytes(int64_t R, int n) {
-    return 2 * al256((uint64_t)R * n * 8) + al256((uint64_t)R * 8) + 4 * al256((uint64_t)R * 4);
+    uint64_t b = 0;
+    for (int k = 0; k < B2N_NSLOT; k++) b += al256((uint64_t)R * b2n_slot_row_bytes(k, n));
+    return b;
 }
 
-static void slot_offsets(int64_t R, int n, int slot, uint64_t off[7]) {
+static void slot_offsets(int64_t R, int n, int slot, uint64_t off[B2N_NSLOT]) {
     uint64_t o = B2N_PEER_HDR + (uint64_t)slot * slot_bytes(R, n);
-    off[0] = o; o += al256((uint64_t)R * n * 8);
-    off[1] = o; o += al256((uint64_t)R * n * 8);
-    off[2] = o; o += al256((uint64_t)R * 8);
-    for (int k = 0; k < 4; k++) { off[3 + k] = o; o += al256((uint64_t)R * 4); }
+    for (int k = 0; k < B2N_NSLOT; k++) { off[k] = o; o += al256((uint64_t)R * b2n_slot_row_bytes(k, n)); }
 }
 
 void b2n_peer_release(b2n_ctx* ctx) {
@@ -135,40 +134,92 @@ int b2n_peer_check(b2n_ctx* ctx) {
 
 }  // extern "C"
 
-int b2n_peer_begin(b2n_ctx* ctx, int n, PeerSet* ps, void** dev7, bool* on) {
+int b2n_chain_begin(b2n_ctx* ctx, const b2n_chain_args* a, bool draw_only, B2nModel* m) {
+    if (!ctx || !a) return B2N_ERR_ARG;
+    if (ctx->start_idx) {
+        ctx->start_idx = nullptr; ctx->start_nrows = 0;
+        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "start rows by index (b2n_set_start_rows) are read by b2n_rwalk_batch only");
+    }
+    if (draw_only) {
+        memset(m, 0, sizeof(*m));
+        m->ndim = a->ndim;
+        m->like_kind = B2N_LIKE_EGGBOX;
+        return B2N_OK;
+    }
+    if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
+    *m = ctx->models[a->model_id];
+    return B2N_OK;
+}
+
+int b2n_chain_none(b2n_ctx* ctx) {
+    return ctx->peer.total > 0 ? b2n_fail(ctx, B2N_ERR_ARG, "gather mode: every rank must run at least one chain") : B2N_OK;
+}
+
+int b2n_chain_dyn(b2n_ctx* ctx, int chains_per_cta) {
+    ctx->dyn.cpc = chains_per_cta;
+    if (!ctx->dyn.plan_only && (ctx->peer.total > 0 || ctx->ptr_mode != B2N_PTR_DEVICE))
+        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
+    return B2N_OK;
+}
+
+int b2n_chain_bind(b2n_ctx* ctx, int n, int64_t Q, void* const* out, void** dev, PeerSet* ps) {
     PeerState& P = ctx->peer;
-    *on = P.total > 0;
     *ps = PeerSet();
-    if (!*on) return B2N_OK;
+    if (P.total == 0) {
+        DevBuf* const stage[B2N_NSLOT] = {&ctx->out0, &ctx->out1, &ctx->out2, &ctx->out3, &ctx->out4, &ctx->out5, &ctx->out6};
+        for (int k = 0; k < B2N_NSLOT; k++) B2N_TRY(b2n_out(ctx, *stage[k], out[k], (size_t)Q * b2n_slot_row_bytes(k, n), &dev[k]));
+        return B2N_OK;
+    }
     if (b2n_peer_window_bytes(P.total, n) > P.win_bytes)
         return b2n_fail(ctx, B2N_ERR_PEER, "exchange window too small for this fill (b2n_peer_window_bytes)");
     P.epoch++;
     slot_offsets(P.total, n, (int)(P.epoch & 1), P.off);
-    const uint64_t rowb[7] = {(uint64_t)n * 8, (uint64_t)n * 8, 8, 4, 4, 4, 4};
-    for (int k = 0; k < 7; k++) dev7[k] = P.win + P.off[k] + (uint64_t)P.row0 * rowb[k];
+    for (int k = 0; k < B2N_NSLOT; k++) dev[k] = P.win + P.off[k] + (uint64_t)P.row0 * b2n_slot_row_bytes(k, n);
     ps->world = P.world;
     ps->rank = P.rank;
     for (int w = 0; w < P.world; w++) ps->base[w] = P.base[w];
     ps->target = (unsigned long long)P.world * P.epoch;
+    if (P.row0 + Q > P.total) return b2n_fail(ctx, B2N_ERR_ARG, "gather rows out of range (b2n_peer_rows)");
     return B2N_OK;
 }
 
-int b2n_peer_end(b2n_ctx* ctx, int n, void* const* user7) {
+__global__ void chain_flags_kernel(const uint32_t* flags, int64_t Q, uint32_t mask, unsigned* out) {
+    uint32_t bad = 0;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < Q; i += (int64_t)gridDim.x * blockDim.x)
+        bad |= flags[i] & mask;
+    if (bad) atomicOr(out, bad);
+}
+
+int b2n_chain_end(b2n_ctx* ctx, int n, int64_t Q, void* const* out, void* const* dev, const B2nFlagStatus* tab,
+                  int ntab) {
     PeerState& P = ctx->peer;
-    const uint64_t rowb[7] = {(uint64_t)n * 8, (uint64_t)n * 8, 8, 4, 4, 4, 4};
-    const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    for (int k = 0; k < 7; k++) {
-        if (!user7[k]) continue;
-        B2N_CUDA(ctx, cudaMemcpyAsync(user7[k], P.win + P.off[k], (size_t)P.total * rowb[k], kind, ctx->stream));
+    const bool gather = P.total > 0;
+    unsigned* hbits = reinterpret_cast<unsigned*>(ctx->pinned);
+    if (ntab > 0) {
+        uint32_t mask = 0;
+        for (int t = 0; t < ntab; t++) mask |= tab[t].bit;
+        *hbits = 0;
+        B2N_CUDA(ctx, ctx->out7.ensure(64));
+        B2N_CUDA(ctx, cudaMemsetAsync(ctx->out7.p, 0, sizeof(unsigned), ctx->stream));
+        // (gather mode: over the rows of ALL ranks, so that every rank returns the same status)
+        const uint32_t* flags = gather ? (const uint32_t*)(P.win + P.off[B2N_SLOT_FLAGS]) : (const uint32_t*)dev[B2N_SLOT_FLAGS];
+        chain_flags_kernel<<<64, 256, 0, ctx->stream>>>(flags, gather ? P.total : Q, mask, ctx->out7.as<unsigned>());
+        B2N_LAUNCH_CHECK(ctx);
+        B2N_CUDA(ctx, cudaMemcpyAsync(hbits, ctx->out7.p, sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
     }
-    if (ctx->ptr_mode == B2N_PTR_HOST)
-        B2N_CUDA(ctx, cudaMemcpyAsync(P.err_host, P.win + 8, 4, cudaMemcpyDeviceToHost, ctx->stream));
-    return B2N_OK;
-}
-
-int b2n_peer_finish(b2n_ctx* ctx, bool on) {
-    B2N_TRY(b2n_finish(ctx));
-    if (on && ctx->ptr_mode == B2N_PTR_HOST && *ctx->peer.err_host)
+    if (gather) {
+        const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+        for (int k = 0; k < B2N_NSLOT; k++)
+            if (out[k]) B2N_CUDA(ctx, cudaMemcpyAsync(out[k], P.win + P.off[k], (size_t)P.total * b2n_slot_row_bytes(k, n), kind, ctx->stream));
+        if (ctx->ptr_mode == B2N_PTR_HOST)
+            B2N_CUDA(ctx, cudaMemcpyAsync(P.err_host, P.win + 8, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    } else {
+        for (int k = 0; k < B2N_NSLOT; k++) B2N_TRY(b2n_out_done(ctx, out[k], dev[k], (size_t)Q * b2n_slot_row_bytes(k, n)));
+    }
+    if (ntab > 0 || ctx->ptr_mode == B2N_PTR_HOST) B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (gather && ctx->ptr_mode == B2N_PTR_HOST && *P.err_host)
         return b2n_fail(ctx, B2N_ERR_PEER, "a peer never arrived at the exchange (timeout in the kernel)");
+    for (int t = 0; t < ntab; t++)
+        if (*hbits & tab[t].bit) return tab[t].msg ? b2n_fail(ctx, tab[t].status, tab[t].msg) : tab[t].status;
     return B2N_OK;
 }

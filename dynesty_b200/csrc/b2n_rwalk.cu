@@ -1091,20 +1091,20 @@ static int rwalk_plan(b2n_ctx* ctx, const B2nModel& m, int n, int nc, int64_t Q,
 extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t walks, double* u,
                                double* v, double* logl, int32_t* n_accept, int32_t* n_reject,
                                int32_t* ncall) {
-    if (!ctx || !a) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
     // start points by index (b2n_set_start_rows): consumed by THIS call, however it ends
     const int32_t* sidx = ctx->start_idx;
     const int64_t srows = ctx->start_nrows;
     ctx->start_idx = nullptr; ctx->start_nrows = 0;
+    B2nModel m;
+    B2N_TRY(b2n_chain_begin(ctx, a, false, &m));
     const bool gather = ctx->peer.total > 0;      // outputs may be NULL in gather mode (b2n_peer_result)
     if (!gather && (!u || !v || !logl || !n_accept || !n_reject || !ncall)) return B2N_ERR_ARG;
-    if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-    const B2nModel m = ctx->models[a->model_id];
     const int n = a->ndim, nc = a->ncdim;
     const int64_t Q = a->nchain;
     if (n != m.ndim || nc < 1 || nc > n || walks < 1 || Q < 0 || !a->u0) return B2N_ERR_ARG;
     if (ctx->bK < 1 || ctx->bn != nc) return b2n_fail(ctx, B2N_ERR_ARG, "resident bound missing or of wrong dimension (b2n_bound_set)");
-    if (Q == 0) return gather ? b2n_fail(ctx, B2N_ERR_ARG, "gather mode: every rank must run at least one chain") : B2N_OK;
+    if (Q == 0) return b2n_chain_none(ctx);
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     ZcScope zc(ctx);          // pinned caller buffers are read / written in place (host-pointer mode)
 
@@ -1112,9 +1112,8 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
     B2N_TRY(rwalk_plan(ctx, m, n, nc, Q, a->dimflags, plan));
     const bool dyn = ctx->dyn.active;        // device-paced launch (b2n_ns.cu): worklist + scalars in HBM
     if (dyn) {
-        ctx->dyn.cpc = plan.chains_per_cta;
+        B2N_TRY(b2n_chain_dyn(ctx, plan.chains_per_cta));
         if (ctx->dyn.plan_only) return B2N_OK;
-        if (gather || ctx->ptr_mode != B2N_PTR_DEVICE) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
     }
     RwalkParams p;
     p.dyn = dyn ? ctx->dyn.dev : nullptr;
@@ -1144,25 +1143,13 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
         fl.assign(a->dimflags, a->dimflags + n);
         B2N_TRY(b2n_in_host(ctx, ctx->in3, fl.data(), fl.size() * sizeof(uint32_t), &dfl));
     }
-    void *du, *dv, *dl, *dna, *dnr, *dncl;
-    void* gdev[7];
-    bool peer_on = false;
-    B2N_TRY(b2n_peer_begin(ctx, n, &p.peer, gdev, &peer_on));
-    if (peer_on) {
-        if (ctx->peer.row0 + Q > ctx->peer.total) return b2n_fail(ctx, B2N_ERR_ARG, "gather rows out of range (b2n_peer_rows)");
-        du = gdev[0]; dv = gdev[1]; dl = gdev[2]; dna = gdev[3]; dnr = gdev[4]; dncl = gdev[5];
-    } else {
-        B2N_TRY(b2n_out(ctx, ctx->out0, u, (size_t)Q * n * sizeof(double), &du));
-        B2N_TRY(b2n_out(ctx, ctx->out1, v, (size_t)Q * n * sizeof(double), &dv));
-        B2N_TRY(b2n_out(ctx, ctx->out2, logl, (size_t)Q * sizeof(double), &dl));
-        B2N_TRY(b2n_out(ctx, ctx->out3, n_accept, (size_t)Q * sizeof(int), &dna));
-        B2N_TRY(b2n_out(ctx, ctx->out4, n_reject, (size_t)Q * sizeof(int), &dnr));
-        B2N_TRY(b2n_out(ctx, ctx->out5, ncall, (size_t)Q * sizeof(int), &dncl));
-    }
+    void* const out[B2N_NSLOT] = {u, v, logl, n_accept, n_reject, ncall, nullptr};
+    void* dev[B2N_NSLOT];
+    B2N_TRY(b2n_chain_bind(ctx, n, Q, out, dev, &p.peer));
     p.u0 = (const double*)du0; p.start = (const int*)dstart; p.order = (const int*)dorder; p.cta = (const int3*)dcta;
     p.dimflags = (const uint32_t*)dfl;
-    p.u = (double*)du; p.v = (double*)dv; p.logl = (double*)dl;
-    p.nacc = (int*)dna; p.nrej = (int*)dnr; p.ncall = (int*)dncl;
+    p.u = (double*)dev[0]; p.v = (double*)dev[1]; p.logl = (double*)dev[2];
+    p.nacc = (int*)dev[3]; p.nrej = (int*)dev[4]; p.ncall = (int*)dev[5];
 
     const unsigned grid = dyn ? (unsigned)ctx->dyn.max_cta : ncta;
     const int KT = plan.KT;
@@ -1215,16 +1202,5 @@ extern "C" int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t wa
 #undef CALL_WARP
 #undef LAUNCH
     B2N_LAUNCH_CHECK(ctx);
-    if (peer_on) {
-        void* const user7[7] = {u, v, logl, n_accept, n_reject, ncall, nullptr};
-        B2N_TRY(b2n_peer_end(ctx, n, user7));
-        return b2n_peer_finish(ctx, true);
-    }
-    B2N_TRY(b2n_out_done(ctx, u, du, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, v, dv, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, logl, dl, (size_t)Q * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, n_accept, dna, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, n_reject, dnr, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, ncall, dncl, (size_t)Q * sizeof(int)));
-    return b2n_finish(ctx);
+    return b2n_chain_end(ctx, n, Q, out, dev, nullptr, 0);
 }

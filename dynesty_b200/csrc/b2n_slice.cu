@@ -18,32 +18,20 @@
 #include <vector>
 
 
-__global__ void any_error_kernel(const uint32_t* flags, int64_t Q, int* out) {
-    int bad = 0;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < Q; i += (int64_t)gridDim.x * blockDim.x)
-        bad |= (flags[i] & 0x80000000u) ? 1 : 0;
-    if (bad) atomicOr(out, 1);
-}
-
 template <bool RANDOM_DIR>
 static int slice_batch_impl(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slices, int32_t doubling, double* u,
                             double* v, double* logl, int32_t* n_expand, int32_t* n_contract, int32_t* ncall,
                             uint32_t* flags) {
-    if (!ctx || !a) return B2N_ERR_ARG;
-    if (ctx->start_idx) {       // b2n_set_start_rows is for the next b2n_rwalk_batch only: do not let it linger
-        ctx->start_idx = nullptr; ctx->start_nrows = 0;
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "start rows by index (b2n_set_start_rows) are read by b2n_rwalk_batch only");
-    }
+    B2nModel m;
+    B2N_TRY(b2n_chain_begin(ctx, a, false, &m));
     const bool gather = ctx->peer.total > 0;      // outputs may be NULL in gather mode (b2n_peer_result)
     if (!gather && (!u || !v || !logl || !n_expand || !n_contract || !ncall || !flags)) return B2N_ERR_ARG;
-    if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-    const B2nModel m = ctx->models[a->model_id];
     const int n = a->ndim;
     const int64_t Q = a->nchain;
     if (n != m.ndim || a->ncdim != n || slices < 1 || Q < 0 || !a->u0)
         return b2n_fail(ctx, B2N_ERR_ARG, "slice samplers need ncdim == ndim (internal_samplers.py:658, 809)");
     if (ctx->bK < 1 || ctx->bn != n) return b2n_fail(ctx, B2N_ERR_ARG, "resident bound missing or of wrong dimension");
-    if (Q == 0) return gather ? b2n_fail(ctx, B2N_ERR_ARG, "gather mode: every rank must run at least one chain") : B2N_OK;
+    if (Q == 0) return b2n_chain_none(ctx);
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     ZcScope zc(ctx);          // pinned caller buffers are read / written in place (host-pointer mode)
     const int npad = (n + 1) & ~1;
@@ -63,9 +51,8 @@ static int slice_batch_impl(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slice
     const size_t smem = fixed + (ax_s ? ax_b : 0) + (pr_s ? pr_b : 0);
     const bool dyn = ctx->dyn.active;        // device-paced launch (b2n_ns.cu)
     if (dyn) {
-        ctx->dyn.cpc = chains_per_cta;
+        B2N_TRY(b2n_chain_dyn(ctx, chains_per_cta));
         if (ctx->dyn.plan_only) return B2N_OK;
-        if (gather || ctx->ptr_mode != B2N_PTR_DEVICE) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
     }
     SliceParams p;
     p.dyn = dyn ? ctx->dyn.dev : nullptr;
@@ -80,25 +67,12 @@ static int slice_batch_impl(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slice
     } else {
         B2N_TRY(b2n_worklist_dev(ctx, Q, a->ell, ctx->bK, chains_per_cta, &dorder, &dcta, &ncta));
     }
-    void *du, *dv, *dl, *dne, *dnc, *dncl, *dfl;
-    void* gdev[7];
-    bool peer_on = false;
-    B2N_TRY(b2n_peer_begin(ctx, n, &p.peer, gdev, &peer_on));
-    if (peer_on) {
-        if (ctx->peer.row0 + Q > ctx->peer.total) return b2n_fail(ctx, B2N_ERR_ARG, "gather rows out of range (b2n_peer_rows)");
-        du = gdev[0]; dv = gdev[1]; dl = gdev[2]; dne = gdev[3]; dnc = gdev[4]; dncl = gdev[5]; dfl = gdev[6];
-    } else {
-        B2N_TRY(b2n_out(ctx, ctx->out0, u, (size_t)Q * n * sizeof(double), &du));
-        B2N_TRY(b2n_out(ctx, ctx->out1, v, (size_t)Q * n * sizeof(double), &dv));
-        B2N_TRY(b2n_out(ctx, ctx->out2, logl, (size_t)Q * sizeof(double), &dl));
-        B2N_TRY(b2n_out(ctx, ctx->out3, n_expand, (size_t)Q * sizeof(int), &dne));
-        B2N_TRY(b2n_out(ctx, ctx->out4, n_contract, (size_t)Q * sizeof(int), &dnc));
-        B2N_TRY(b2n_out(ctx, ctx->out5, ncall, (size_t)Q * sizeof(int), &dncl));
-        B2N_TRY(b2n_out(ctx, ctx->out6, flags, (size_t)Q * sizeof(uint32_t), &dfl));
-    }
+    void* const out[B2N_NSLOT] = {u, v, logl, n_expand, n_contract, ncall, flags};
+    void* dev[B2N_NSLOT];
+    B2N_TRY(b2n_chain_bind(ctx, n, Q, out, dev, &p.peer));
     p.u0 = (const double*)du0; p.order = (const int*)dorder; p.cta = (const int3*)dcta;
-    p.u = (double*)du; p.v = (double*)dv; p.logl = (double*)dl;
-    p.nexp = (int*)dne; p.ncon = (int*)dnc; p.ncall = (int*)dncl; p.flags = (uint32_t*)dfl;
+    p.u = (double*)dev[0]; p.v = (double*)dev[1]; p.logl = (double*)dev[2];
+    p.nexp = (int*)dev[3]; p.ncon = (int*)dev[4]; p.ncall = (int*)dev[5]; p.flags = (uint32_t*)dev[6];
     const unsigned grid = dyn ? (unsigned)ctx->dyn.max_cta : ncta;
 #define LAUNCH(L, AXS, PRS)                                                                          \
     do {                                                                                             \
@@ -123,35 +97,9 @@ static int slice_batch_impl(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slice
 #undef LAUNCH
     B2N_LAUNCH_CHECK(ctx);
     if (dyn) return B2N_OK;      // device-paced: the commit kernel of the round folds the flags
-    // error summary (a collapsed interval anywhere = RuntimeError in the reference)
-    int* derr = reinterpret_cast<int*>(ctx->pinned);
-    *derr = 0;
-    B2N_CUDA(ctx, ctx->out7.ensure(64));
-    B2N_CUDA(ctx, cudaMemsetAsync(ctx->out7.p, 0, sizeof(int), ctx->stream));
-    // (gather mode: over the rows of ALL ranks, so that every rank raises the same error)
-    const uint32_t* eflags = peer_on ? (const uint32_t*)(ctx->peer.win + ctx->peer.off[6]) : (const uint32_t*)dfl;
-    any_error_kernel<<<64, 256, 0, ctx->stream>>>(eflags, peer_on ? ctx->peer.total : Q, ctx->out7.as<int>());
-    B2N_LAUNCH_CHECK(ctx);
-    B2N_CUDA(ctx, cudaMemcpyAsync(derr, ctx->out7.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (peer_on) {
-        void* const user7[7] = {u, v, logl, n_expand, n_contract, ncall, flags};
-        B2N_TRY(b2n_peer_end(ctx, n, user7));
-        B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (ctx->ptr_mode == B2N_PTR_HOST && *ctx->peer.err_host)
-            return b2n_fail(ctx, B2N_ERR_PEER, "a peer never arrived at the exchange (timeout in the kernel)");
-        if (*derr) return B2N_ERR_SLICE_FAIL;
-        return B2N_OK;
-    }
-    B2N_TRY(b2n_out_done(ctx, u, du, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, v, dv, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, logl, dl, (size_t)Q * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, n_expand, dne, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, n_contract, dnc, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, ncall, dncl, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, flags, dfl, (size_t)Q * sizeof(uint32_t)));
-    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // the error word is a host result
-    if (*derr) return B2N_ERR_SLICE_FAIL;
-    return B2N_OK;
+    // a collapsed interval anywhere = RuntimeError in the reference
+    static const B2nFlagStatus fail[] = {{0x80000000u, B2N_ERR_SLICE_FAIL, nullptr}};
+    return b2n_chain_end(ctx, n, Q, out, dev, fail, 1);
 }
 
 extern "C" int b2n_rslice_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slices, int32_t doubling,

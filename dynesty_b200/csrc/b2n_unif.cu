@@ -12,41 +12,27 @@
 #include <vector>
 
 
-__global__ void unif_error_kernel(const uint32_t* flags, int64_t Q, int* out) {
-    int bad = 0;
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < Q; i += (int64_t)gridDim.x * blockDim.x) {
-        if (flags[i] & 0x40000000u) bad |= 1;
-        if (flags[i] & 0x80000000u) bad |= 2;
-    }
-    if (bad) atomicOr(out, bad);
-}
-
 extern "C" int b2n_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, double* v, double* logl,
                               int32_t* ncall, int32_t* nprop, uint32_t* flags) {
-    if (!ctx || !a) return B2N_ERR_ARG;
-    if (ctx->start_idx) {       // b2n_set_start_rows is for the next b2n_rwalk_batch only: do not let it linger
-        ctx->start_idx = nullptr; ctx->start_nrows = 0;
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "start rows by index (b2n_set_start_rows) are read by b2n_rwalk_batch only");
-    }
+    B2nModel m;
+    B2N_TRY(b2n_chain_begin(ctx, a, a && (a->reserved & B2N_OPT_DRAW_ONLY), &m));
+    const int draw_only = (a->reserved & B2N_OPT_DRAW_ONLY) ? ((a->reserved & B2N_OPT_DRAW_MIXTURE) ? 3 : 1) : 0;
     const bool gather = ctx->peer.total > 0;      // outputs may be NULL in gather mode (b2n_peer_result)
     if (!gather && (!u || !v || !logl || !ncall || !nprop || !flags)) return B2N_ERR_ARG;
-    const int draw_only = (a->reserved & B2N_OPT_DRAW_ONLY) ? ((a->reserved & B2N_OPT_DRAW_MIXTURE) ? 3 : 1) : 0;
-    B2nModel m;
-    memset(&m, 0, sizeof(m));
-    m.ndim = a->ndim;
-    m.like_kind = B2N_LIKE_EGGBOX;
-    if (!draw_only) {
-        if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-        m = ctx->models[a->model_id];
-    }
     const int n = a->ndim, nc = a->ncdim;
     const int64_t Q = a->nchain;
     if (n != m.ndim || nc < 1 || nc > n || Q < 0 || (draw_only && n != nc)) return B2N_ERR_ARG;
     if (ctx->bK < 1 || ctx->bn != nc || ctx->h_logvols.empty())
         return b2n_fail(ctx, B2N_ERR_ARG, "resident bound (with ctrs/ams/logvols) missing or of wrong dimension");
-    if (Q == 0) return gather ? b2n_fail(ctx, B2N_ERR_ARG, "gather mode: every rank must run at least one chain") : B2N_OK;
+    if (Q == 0) return b2n_chain_none(ctx);
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     ZcScope zc(ctx);          // pinned caller buffers are written in place (host-pointer mode)
+    const bool dyn = ctx->dyn.active;        // device-paced launch (b2n_ns.cu)
+    if (dyn) {
+        B2N_TRY(b2n_chain_dyn(ctx, 1));
+        if (ctx->dyn.plan_only) return B2N_OK;
+        if (draw_only) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
+    }
     const int K = ctx->bK;
     // probs = exp(logvol_ells - logsumexp(logvol_ells)) ; cumsum (bounding.py:552, 1305)
     std::vector<double> cum(K);
@@ -64,32 +50,17 @@ extern "C" int b2n_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, 
         fl.assign(a->dimflags, a->dimflags + n);
         B2N_TRY(b2n_in_host(ctx, ctx->in3, fl.data(), fl.size() * sizeof(uint32_t), &dfl_in));
     }
-    const bool dyn = ctx->dyn.active;        // device-paced launch (b2n_ns.cu)
-    if (dyn && (gather || ctx->ptr_mode != B2N_PTR_DEVICE || draw_only))
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
     UnifParams p;
     p.dyn = dyn ? ctx->dyn.dev : nullptr;
     p.m = m; p.n = n; p.nc = nc; p.K = K; p.Q = Q; p.draw_only = draw_only;
     p.ctrs = ctx->b_ctrs.as<double>(); p.ams = ctx->b_ams.as<double>(); p.axesT = ctx->b_axesT.as<double>();
     p.cum = (const double*)dcum; p.dimflags = (const uint32_t*)dfl_in;
     p.loglstar = a->loglstar; p.seed = a->seed; p.chain0 = a->chain0;
-    void *du, *dv, *dl, *dnc, *dnp, *dfl;
-    void* gdev[7];
-    bool peer_on = false;
-    B2N_TRY(b2n_peer_begin(ctx, n, &p.peer, gdev, &peer_on));
-    if (peer_on) {
-        if (ctx->peer.row0 + Q > ctx->peer.total) return b2n_fail(ctx, B2N_ERR_ARG, "gather rows out of range (b2n_peer_rows)");
-        du = gdev[0]; dv = gdev[1]; dl = gdev[2]; dnc = gdev[3]; dnp = gdev[4]; dfl = gdev[6];
-    } else {
-        B2N_TRY(b2n_out(ctx, ctx->out0, u, (size_t)Q * n * sizeof(double), &du));
-        B2N_TRY(b2n_out(ctx, ctx->out1, v, (size_t)Q * n * sizeof(double), &dv));
-        B2N_TRY(b2n_out(ctx, ctx->out2, logl, (size_t)Q * sizeof(double), &dl));
-        B2N_TRY(b2n_out(ctx, ctx->out3, ncall, (size_t)Q * sizeof(int), &dnc));
-        B2N_TRY(b2n_out(ctx, ctx->out4, nprop, (size_t)Q * sizeof(int), &dnp));
-        B2N_TRY(b2n_out(ctx, ctx->out6, flags, (size_t)Q * sizeof(uint32_t), &dfl));
-    }
-    p.u = (double*)du; p.v = (double*)dv; p.logl = (double*)dl;
-    p.ncall = (int*)dnc; p.nprop = (int*)dnp; p.flags = (uint32_t*)dfl;
+    void* const out[B2N_NSLOT] = {u, v, logl, ncall, nprop, nullptr, flags};
+    void* dev[B2N_NSLOT];
+    B2N_TRY(b2n_chain_bind(ctx, n, Q, out, dev, &p.peer));
+    p.u = (double*)dev[0]; p.v = (double*)dev[1]; p.logl = (double*)dev[2];
+    p.ncall = (int*)dev[3]; p.nprop = (int*)dev[4]; p.flags = (uint32_t*)dev[6];
     const int threads = 128, wpb = threads / 32;
     const size_t smem = (size_t)wpb * 5 * n * sizeof(double);
     if (smem > (size_t)ctx->max_smem_optin) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the unif kernel");
@@ -109,79 +80,41 @@ extern "C" int b2n_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, 
 #undef CALL
     B2N_LAUNCH_CHECK(ctx);
     if (dyn) return B2N_OK;      // device-paced: the commit kernel of the round folds the flags
-    int* herr = reinterpret_cast<int*>(ctx->pinned);
-    *herr = 0;
-    B2N_CUDA(ctx, ctx->out7.ensure(64));
-    B2N_CUDA(ctx, cudaMemsetAsync(ctx->out7.p, 0, sizeof(int), ctx->stream));
-    const uint32_t* eflags = peer_on ? (const uint32_t*)(ctx->peer.win + ctx->peer.off[6]) : (const uint32_t*)dfl;
-    unif_error_kernel<<<64, 256, 0, ctx->stream>>>(eflags, peer_on ? ctx->peer.total : Q, ctx->out7.as<int>());
-    B2N_LAUNCH_CHECK(ctx);
-    B2N_CUDA(ctx, cudaMemcpyAsync(herr, ctx->out7.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (peer_on) {
-        void* const user7[7] = {u, v, logl, ncall, nprop, nullptr, flags};
-        B2N_TRY(b2n_peer_end(ctx, n, user7));
-        B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (ctx->ptr_mode == B2N_PTR_HOST && *ctx->peer.err_host)
-            return b2n_fail(ctx, B2N_ERR_PEER, "a peer never arrived at the exchange (timeout in the kernel)");
-        if (*herr & 1) return B2N_ERR_Q0;
-        if (*herr & 2) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "uniform sampling did not find a point (bound draw limit)");
-        return B2N_OK;
-    }
-    B2N_TRY(b2n_out_done(ctx, u, du, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, v, dv, (size_t)Q * n * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, logl, dl, (size_t)Q * sizeof(double)));
-    B2N_TRY(b2n_out_done(ctx, ncall, dnc, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, nprop, dnp, (size_t)Q * sizeof(int)));
-    B2N_TRY(b2n_out_done(ctx, flags, dfl, (size_t)Q * sizeof(uint32_t)));
-    B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*herr & 1) return B2N_ERR_Q0;
-    if (*herr & 2) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "uniform sampling did not find a point (bound draw limit)");
-    return B2N_OK;
+    static const B2nFlagStatus fail[] = {
+        {0x40000000u, B2N_ERR_Q0, nullptr},
+        {0x80000000u, B2N_ERR_UNSUPPORTED, "uniform sampling did not find a point (bound draw limit)"}};
+    return b2n_chain_end(ctx, n, Q, out, dev, fail, 2);
 }
 
 
 extern "C" int b2n_unitcube_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, double* v, double* logl,
                                   int32_t* ncall, uint32_t* flags) {
-    if (!ctx || !a) return B2N_ERR_ARG;
-    if (ctx->start_idx) {       // b2n_set_start_rows is for the next b2n_rwalk_batch only: do not let it linger
-        ctx->start_idx = nullptr; ctx->start_nrows = 0;
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "start rows by index (b2n_set_start_rows) are read by b2n_rwalk_batch only");
-    }
+    B2nModel m;
+    B2N_TRY(b2n_chain_begin(ctx, a, false, &m));
     const bool gather = ctx->peer.total > 0;
     if (!gather && (!u || !v || !logl || !ncall)) return B2N_ERR_ARG;
-    if (a->model_id < 0 || a->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-    const B2nModel m = ctx->models[a->model_id];
     const int n = a->ndim;
     const int64_t Q = a->nchain;
     if (n != m.ndim || Q < 0) return B2N_ERR_ARG;
-    if (Q == 0) return gather ? b2n_fail(ctx, B2N_ERR_ARG, "gather mode: every rank must run at least one chain") : B2N_OK;
+    if (Q == 0) return b2n_chain_none(ctx);
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     ZcScope zc(ctx);
     const bool dyn = ctx->dyn.active;
     if (dyn) {
-        ctx->dyn.cpc = 1;
+        B2N_TRY(b2n_chain_dyn(ctx, 1));
         if (ctx->dyn.plan_only) return B2N_OK;
-        if (gather || ctx->ptr_mode != B2N_PTR_DEVICE) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "device-paced launch needs device pointers and no gather mode");
     }
     CubeParams p;
     p.dyn = dyn ? ctx->dyn.dev : nullptr;
     p.m = m; p.n = n; p.Q = Q; p.loglstar = a->loglstar; p.seed = a->seed; p.chain0 = a->chain0;
-    void *du, *dv, *dl, *dnc, *dfl = nullptr;
-    void* gdev[7];
-    bool peer_on = false;
-    B2N_TRY(b2n_peer_begin(ctx, n, &p.peer, gdev, &peer_on));
-    if (peer_on) {
-        if (ctx->peer.row0 + Q > ctx->peer.total) return b2n_fail(ctx, B2N_ERR_ARG, "gather rows out of range (b2n_peer_rows)");
-        du = gdev[0]; dv = gdev[1]; dl = gdev[2]; dnc = gdev[3]; dfl = gdev[6];
-    } else {
-        B2N_TRY(b2n_out(ctx, ctx->out0, u, (size_t)Q * n * sizeof(double), &du));
-        B2N_TRY(b2n_out(ctx, ctx->out1, v, (size_t)Q * n * sizeof(double), &dv));
-        B2N_TRY(b2n_out(ctx, ctx->out2, logl, (size_t)Q * sizeof(double), &dl));
-        B2N_TRY(b2n_out(ctx, ctx->out3, ncall, (size_t)Q * sizeof(int), &dnc));
-        if (dyn) dfl = flags;
-        else { B2N_CUDA(ctx, ctx->out6.ensure((size_t)Q * sizeof(uint32_t))); dfl = ctx->out6.p; }
+    void* const out[B2N_NSLOT] = {u, v, logl, ncall, nullptr, nullptr, flags};
+    void* dev[B2N_NSLOT];
+    B2N_TRY(b2n_chain_bind(ctx, n, Q, out, dev, &p.peer));
+    if (!dev[B2N_SLOT_FLAGS]) {      // flags may be NULL: the draw-limit summary still reads them
+        B2N_CUDA(ctx, ctx->out6.ensure((size_t)Q * sizeof(uint32_t)));
+        dev[B2N_SLOT_FLAGS] = ctx->out6.p;
     }
-    p.u = (double*)du; p.v = (double*)dv; p.logl = (double*)dl; p.ncall = (int*)dnc; p.flags = (uint32_t*)dfl;
+    p.u = (double*)dev[0]; p.v = (double*)dev[1]; p.logl = (double*)dev[2]; p.ncall = (int*)dev[3]; p.flags = (uint32_t*)dev[6];
     const int threads = 128, wpb = threads / 32;
     const size_t smem = (size_t)wpb * 3 * n * sizeof(double);
     if (smem > (size_t)ctx->max_smem_optin) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "ndim too large for the unit-cube kernel");
@@ -201,29 +134,7 @@ extern "C" int b2n_unitcube_batch(b2n_ctx* ctx, const b2n_chain_args* a, double*
 #undef CALL
     B2N_LAUNCH_CHECK(ctx);
     if (dyn) return B2N_OK;
-    int* herr = reinterpret_cast<int*>(ctx->pinned);
-    *herr = 0;
-    B2N_CUDA(ctx, ctx->out7.ensure(64));
-    B2N_CUDA(ctx, cudaMemsetAsync(ctx->out7.p, 0, sizeof(int), ctx->stream));
-    const uint32_t* eflags = peer_on ? (const uint32_t*)(ctx->peer.win + ctx->peer.off[6]) : (const uint32_t*)dfl;
-    unif_error_kernel<<<64, 256, 0, ctx->stream>>>(eflags, peer_on ? ctx->peer.total : Q, ctx->out7.as<int>());
-    B2N_LAUNCH_CHECK(ctx);
-    B2N_CUDA(ctx, cudaMemcpyAsync(herr, ctx->out7.p, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (peer_on) {
-        void* const user7[7] = {u, v, logl, ncall, nullptr, nullptr, flags};
-        B2N_TRY(b2n_peer_end(ctx, n, user7));
-        B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (ctx->ptr_mode == B2N_PTR_HOST && *ctx->peer.err_host)
-            return b2n_fail(ctx, B2N_ERR_PEER, "a peer never arrived at the exchange (timeout in the kernel)");
-    } else {
-        B2N_TRY(b2n_out_done(ctx, u, du, (size_t)Q * n * sizeof(double)));
-        B2N_TRY(b2n_out_done(ctx, v, dv, (size_t)Q * n * sizeof(double)));
-        B2N_TRY(b2n_out_done(ctx, logl, dl, (size_t)Q * sizeof(double)));
-        B2N_TRY(b2n_out_done(ctx, ncall, dnc, (size_t)Q * sizeof(int)));
-        if (flags && ctx->ptr_mode == B2N_PTR_HOST)
-            B2N_CUDA(ctx, cudaMemcpyAsync(flags, dfl, (size_t)Q * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-        B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    if (*herr & 2) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "unit-cube sampling did not find a point above the threshold (draw limit)");
-    return B2N_OK;
+    static const B2nFlagStatus fail[] = {
+        {0x80000000u, B2N_ERR_UNSUPPORTED, "unit-cube sampling did not find a point above the threshold (draw limit)"}};
+    return b2n_chain_end(ctx, n, Q, out, dev, fail, 1);
 }

@@ -197,10 +197,8 @@ def friends_unif_batch(model, nchain, ndim, loglstar, seed, chain0=0, dimflags=N
     a, keep, Q, n = _chain_args(model, None, ndim, loglstar, 1.0, seed, chain0, None, dimflags, Q=int(nchain), ndim=int(ndim))
     if draw_only:
         a.reserved = 3 if mixture else 1
-    o = dict(u=np.empty((Q, n)), v=np.empty((Q, n)), logl=np.empty(Q), ncall=np.empty(Q, dtype=np.int32),
-             nprop=np.empty(Q, dtype=np.int32), flags=np.empty(Q, dtype=np.uint32))
-    ctx.check(ctx.lib.b2n_friends_unif_batch(ctx.h, C.byref(a), ptr(o['u']), ptr(o['v']), ptr(o['logl']), ptr(o['ncall']),
-                                             ptr(o['nprop']), ptr(o['flags'])))
+    o = _chain_outputs('unif', Q, n)
+    ctx.check(ctx.lib.b2n_friends_unif_batch(ctx.h, C.byref(a), *_chain_ptrs(o, 'unif')))
     if not draw_only and (o['flags'] & 0x80000000).any():
         raise NotImplementedError("uniform sampling did not find a point (bound draw limit)")
     return o
@@ -264,6 +262,26 @@ def dimflags_from(ndim, periodic=None, reflective=None):
     return f
 
 
+def _chain_outputs(sampler, R, n):
+    """Fresh output arrays of R chains of `sampler` (_lib.CHAIN_OUTPUTS), keyed as the sampler returns them."""
+    o = dict(u=np.empty((R, n)), v=np.empty((R, n)), logl=np.empty(R))
+    for nm in _lib.CHAIN_OUTPUTS[sampler]:
+        if nm is not None:
+            o[nm] = np.empty(R, dtype=np.uint32 if nm == 'flags' else np.int32)
+    return o
+
+
+# the output arguments of each sampler's entry point, in order (names built once: rwalk_batch is on the timed path)
+_CHAIN_ARGS = {s: ('u', 'v', 'logl') + tuple(nm for nm in names if nm is not None)
+               for s, names in _lib.CHAIN_OUTPUTS.items()}
+
+
+def _chain_ptrs(o, sampler):
+    """The output arguments of the sampler's entry point: addresses of o's arrays (NULL where o has none)."""
+    g = o.get
+    return [ptr(g(nm)) for nm in _CHAIN_ARGS[sampler]]
+
+
 class _gather:
     """Context manager for the fused multi-GPU gather (include/b200nest.h, peer section):
     `peer = (row0, total_rows)` makes the chains of the call rows [row0, row0 + Q) of a
@@ -304,15 +322,9 @@ def rwalk_batch(model, u0, loglstar, scale, walks, seed, chain0=0, ncdim=None, e
         ctx.set_start_rows(ptr(start_rows), Q)          # Q rows of u0 = the live set
         Q = a.nchain
     R = Q if peer is None else int(peer[1])
-    o = out if out is not None else dict(
-        u=np.empty((R, n)), v=np.empty((R, n)), logl=np.empty(R),
-        n_accept=np.empty(R, dtype=np.int32), n_reject=np.empty(R, dtype=np.int32),
-        ncall=np.empty(R, dtype=np.int32))
-    g = o.get
+    o = out if out is not None else _chain_outputs('rwalk', R, n)
     with _gather(ctx, peer):
-        ctx.check(ctx.lib.b2n_rwalk_batch(ctx.h, C.byref(a), int(walks), ptr(g('u')), ptr(g('v')),
-                                          ptr(g('logl')), ptr(g('n_accept')), ptr(g('n_reject')),
-                                          ptr(g('ncall'))))
+        ctx.check(ctx.lib.b2n_rwalk_batch(ctx.h, C.byref(a), int(walks), *_chain_ptrs(o, 'rwalk')))
     return o
 
 
@@ -320,13 +332,9 @@ def _slice_batch(fn, model, u0, loglstar, scale, slices, seed, chain0, doubling,
     ctx = _ctx(ctx)
     a, keep, Q, n = _chain_args(model, u0, None, loglstar, scale, seed, chain0, ell, None)
     R = Q if peer is None else int(peer[1])
-    o = dict(u=np.empty((R, n)), v=np.empty((R, n)), logl=np.empty(R),
-             n_expand=np.empty(R, dtype=np.int32), n_contract=np.empty(R, dtype=np.int32),
-             ncall=np.empty(R, dtype=np.int32), flags=np.empty(R, dtype=np.uint32))
+    o = _chain_outputs('slice', R, n)
     with _gather(ctx, peer):
-        ctx.check(getattr(ctx.lib, fn)(ctx.h, C.byref(a), int(slices), int(bool(doubling)), ptr(o['u']),
-                                       ptr(o['v']), ptr(o['logl']), ptr(o['n_expand']), ptr(o['n_contract']),
-                                       ptr(o['ncall']), ptr(o['flags'])))
+        ctx.check(getattr(ctx.lib, fn)(ctx.h, C.byref(a), int(slices), int(bool(doubling)), *_chain_ptrs(o, 'slice')))
     return o
 
 
@@ -354,11 +362,9 @@ def unif_batch(model, nchain, ndim, loglstar, seed, chain0=0, ncdim=None, dimfla
     if draw_only:
         a.reserved = 3 if mixture else 1      # mixture: no 1/q test, q returned in 'ncall'
     R = Q if peer is None else int(peer[1])
-    o = dict(u=np.empty((R, n)), v=np.empty((R, n)), logl=np.empty(R), ncall=np.empty(R, dtype=np.int32),
-             nprop=np.empty(R, dtype=np.int32), flags=np.empty(R, dtype=np.uint32))
+    o = _chain_outputs('unif', R, n)
     with _gather(ctx, peer):
-        ctx.check(ctx.lib.b2n_unif_batch(ctx.h, C.byref(a), ptr(o['u']), ptr(o['v']), ptr(o['logl']),
-                                         ptr(o['ncall']), ptr(o['nprop']), ptr(o['flags'])))
+        ctx.check(ctx.lib.b2n_unif_batch(ctx.h, C.byref(a), *_chain_ptrs(o, 'unif')))
     return o
 
 
@@ -367,10 +373,9 @@ def unitcube_batch(model, nchain, ndim, loglstar, seed, chain0=0, ctx=None, peer
     ctx = _ctx(ctx)
     a, keep, Q, n = _chain_args(model, None, None, loglstar, 1.0, seed, chain0, None, None, Q=int(nchain), ndim=int(ndim))
     R = Q if peer is None else int(peer[1])
-    o = dict(u=np.empty((R, n)), v=np.empty((R, n)), logl=np.empty(R), ncall=np.empty(R, dtype=np.int32))
+    o = _chain_outputs('unitcube', R, n)
     with _gather(ctx, peer):
-        ctx.check(ctx.lib.b2n_unitcube_batch(ctx.h, C.byref(a), ptr(o['u']), ptr(o['v']), ptr(o['logl']),
-                                             ptr(o['ncall']), None))
+        ctx.check(ctx.lib.b2n_unitcube_batch(ctx.h, C.byref(a), *_chain_ptrs(o, 'unitcube'), None))
     return o
 
 

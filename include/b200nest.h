@@ -499,8 +499,11 @@ int b2n_friends_unif_batch(b2n_ctx* ctx, const b2n_chain_args* a, double* u, dou
  *                     device-pointer mode: read the window through b2n_peer_result instead).
  *                     total_rows = 0 switches gather mode off.  All ranks must issue the same
  *                     sequence of gather-mode calls.
- *   b2n_peer_result   window pointer + byte offsets {u, v, logl, int0, int1, int2, int3} of the
- *                     last gather-mode call (int0..3 = the call's int32 outputs in argument order)
+ *   b2n_peer_result   window pointer + byte offsets {u, v, logl, int0, int1, int2, flags} of the
+ *                     last gather-mode call.  int0..int2 hold the call's int32 counters in argument
+ *                     order, flags its uint32 flags: rwalk n_accept, n_reject, ncall; slice
+ *                     n_expand, n_contract, ncall, flags; unif ncall, nprop, -, flags; unitcube
+ *                     ncall, -, -, flags.
  *   b2n_peer_read     synchronise and copy `bytes` at byte `offset` of the own window to HOST memory
  *   b2n_peer_check    synchronise and report B2N_ERR_PEER if a peer never arrived (device mode;
  *                     host-pointer mode checks on return of every call).

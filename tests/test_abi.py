@@ -62,6 +62,22 @@ def test_pure_host_entry_points(lib):
     assert l.b2n_peer_window_bytes(2000, 50) == 256 + 2 * (2 * al(2000 * 50 * 8) + al(2000 * 8) + 4 * al(2000 * 4))
 
 
+CHAIN_ENTRY_POINTS = ['b2n_rwalk_batch', 'b2n_rslice_batch', 'b2n_slice_batch', 'b2n_unif_batch',
+                      'b2n_unitcube_batch', 'b2n_friends_unif_batch']
+
+
+@pytest.mark.parametrize('name', CHAIN_ENTRY_POINTS)
+def test_chain_entry_points_refuse_a_null_ctx(name):
+    """A chain entry point answers a NULL ctx with B2N_ERR_ARG before it touches CUDA, whether or not it is given
+    its arguments (the NULL-args case with a live ctx is in tests/test_gpu_chain_entry.py)."""
+    l = _lib.load()
+    argtypes = _lib.SYMBOLS[name][1]
+    rest = [0 if t is _lib._I else None for t in argtypes[2:]]
+    a = _lib.ChainArgs()
+    assert getattr(l, name)(None, C.byref(a), *rest) == _lib.ERR_ARG
+    assert getattr(l, name)(None, None, *rest) == _lib.ERR_ARG
+
+
 def test_product_path_fails_loudly_without_a_gpu():
     try:
         import torch

@@ -66,7 +66,7 @@ def test_peer_world1_rwalk_rows(name):
     ctx.close()
 
 
-@pytest.mark.parametrize('kind', ['rslice', 'slice', 'unif'])
+@pytest.mark.parametrize('kind', ['rslice', 'slice', 'unif', 'unitcube'])
 def test_peer_world1_slice_unif(kind):
     m, dm, e, u0, loglstar = _setup('g6')
     Q, n = u0.shape
@@ -76,11 +76,16 @@ def test_peer_world1_slice_unif(kind):
     mid = dm.model_id(ctx)
     if kind == 'unif':
         run = lambda **kw: ops.unif_batch(mid, Q, n, loglstar, 3, chain0=70, ctx=ctx, **kw)
+    elif kind == 'unitcube':          # prior draws: a threshold half of them pass
+        prior = np.random.default_rng(1).random((1000, n))
+        lcube = float(np.median(m.loglike(m.prior_transform(prior))))
+        run = lambda **kw: ops.unitcube_batch(mid, Q, n, lcube, 3, chain0=70, ctx=ctx, **kw)
     else:
         fn = ops.rslice_batch if kind == 'rslice' else ops.slice_batch
         run = lambda **kw: fn(mid, u0, loglstar, 0.8, 4, 3, chain0=70, ctx=ctx, **kw)
     ref = run()
     o = run(peer=(row0, total))
+    assert o.keys() == ref.keys()
     for k in ref:
         assert np.array_equal(o[k][row0:row0 + Q], ref[k]), k
     ctx.close()
