@@ -236,34 +236,47 @@ __device__ __forceinline__ void ball_direction_pair_fast(const ChainRng& ga, con
     fb = b2n_div(exp(lb * inv_nc), b2n_sqrt(two ? ssb : 1.0));
 }
 
-// One direction with the branch-free math, WITHOUT the step factor: z -> b2n_sm[off..] (when `store`), returns the
-// warp-reduced |z|^2 and log(U) of the radius uniform (lane 31's block, see ball_direction).  The caller forms
-// U^(1/nc) / |z| later -- the draw warps of rwalk_mmaws_kernel do that for a whole ring of items at once, one LANE
-// per item, instead of once per item on all 32 lanes.  Same draw events, ticks and arithmetic as ball_direction_pair_fast.
-__device__ __forceinline__ void ball_draw_fast(const ChainRng& g, int off, bool store, int nc, int lane, double& ss,
-                                               double& lgU) {
+// ONE Philox block of a direction draw with the branch-free math, for callers that deal the blocks of many directions
+// over the lanes (the draw warps of rwalk_mmaws_kernel).  j < nb = (nc + 1) / 2: Box-Muller block j of the normal
+// vector event -> z[2j], z[2j + 1] at b2n_sm[off + 2j..], and its share of |z|^2 (the expression ball_direction's
+// lane j forms) -> b2n_sm[osc].  j == nb: the block of the radius uniform (the one ball_direction's lane 31 draws)
+// -> log U at b2n_sm[osc]; it runs the same straight-line code and stores only the log.  Nothing is stored unless `store`.
+__device__ __forceinline__ void ball_block_fast(const ChainRng& g, int j, int nc, int off, int osc, bool store) {
     const int nb = (nc + 1) >> 1;
-    const bool isr = lane == 31;
-    const uint4 r = curand_Philox4x32_10(make_uint4(isr ? 0u : (uint32_t)lane, g.tick + (isr ? 1u : 0u), g.c2, g.c3),
+    const bool isr = j == nb;
+    const uint4 r = curand_Philox4x32_10(make_uint4(isr ? 0u : (uint32_t)j, g.tick + (isr ? 1u : 0u), g.c2, g.c3),
                                          g.key);
     const double lg = b2n_log(b2n_u52(r.x, r.y));
     const double rad = b2n_sqrt(-2.0 * lg);
     double sn, cs;
     b2n_sincos2pi(b2n_u52(r.z, r.w), &sn, &cs);
     const double z0 = rad * cs, z1 = rad * sn;
-    double s = 0.0;
-    if (lane < nb) {
-        const bool full = 2 * lane + 1 < nc;
-        s = full ? fma(z1, z1, z0 * z0) : z0 * z0;
-        if (store) {
-            if (full) *reinterpret_cast<double2*>(&b2n_sm[off + 2 * lane]) = make_double2(z0, z1);
-            else b2n_sm[off + 2 * lane] = z0;
+    if (store) {
+        const bool full = 2 * j + 1 < nc;
+        if (isr) {
+            b2n_sm[osc] = lg;
+        } else if (full) {
+            *reinterpret_cast<double2*>(&b2n_sm[off + 2 * j]) = make_double2(z0, z1);
+            b2n_sm[osc] = fma(z1, z1, z0 * z0);
+        } else {
+            b2n_sm[off + 2 * j] = z0;
+            b2n_sm[osc] = z0 * z0;
         }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(B2N_FULL, s, o);
-    ss = s;
-    lgU = __shfl_sync(B2N_FULL, lg, 31);
+}
+
+// |z|^2 from the per-block shares s[j] = b2n_sm[o + j], j < nb (<= 31), on ONE lane, summed in the association of the
+// 32-lane butterfly `for (o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(.., s, o)` over lanes holding s[lane] (0.0 from
+// lane nb on): node(a, m) = node(a, 2m) + node(a + m, 2m), leaves s[a] + s[a + 16].  Floating-point addition is
+// commutative, so every lane of that butterfly holds exactly this value.
+template <int M>
+__device__ __forceinline__ double ss_butterfly(int o, int nb, int a) {
+    if constexpr (M == 16) {
+        const double lo = a < nb ? b2n_sm[o + a] : 0.0, hi = a + 16 < nb ? b2n_sm[o + a + 16] : 0.0;
+        return lo + hi;
+    } else {
+        return ss_butterfly<2 * M>(o, nb, a) + ss_butterfly<2 * M>(o, nb, a + M);
+    }
 }
 
 // Stage a column-major matrix (n x n, ld = n in global) into b2n_sm with padded leading dim.

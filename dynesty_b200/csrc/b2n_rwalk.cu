@@ -293,15 +293,21 @@ __global__ void __launch_bounds__(256, 2) rwalk_mma_kernel(const RwalkParams p) 
 // barriers that leave the schedulers idle most of the time.  The draws of a step do not depend on the chain state, so
 // they do not have to sit in the same instruction stream at all:
 //   * warps 8..11 (one per scheduler) do nothing but draw: they fill a DOUBLE-BUFFERED ring of directions (8 steps x 8
-//     chains per buffer) one buffer ahead of the step warps and issue into the cycles the step warps leave empty;
-//     the step factors scale * U^(1/n) / |z| of a buffer are formed with one LANE per ring slot;
+//     chains per buffer) one buffer ahead of the step warps and issue into the cycles the step warps leave empty.
+//     A draw warp deals the Philox blocks of its items -- nb = (n + 1) / 2 Box-Muller pair blocks and one radius block
+//     each -- over its lanes as ONE flat space, one block per lane and two side by side, so no lane draws a block
+//     nobody uses (a warp per item leaves 32 - nb - 1 lanes idle: 6 at n = 50, 15 at n = 32); each block leaves its
+//     share of |z|^2 (or log U) in the warp's scratch, and one LANE per item then sums |z|^2 in the association of
+//     the former 32-lane butterfly (ss_butterfly: bit-identical) and forms the step factor scale * U^(1/n) / |z|;
 //   * warps 0..7 run the step phases of rwalk_mma_kernel on register-resident DMMA fragments, with every shared-memory
 //     offset a compile-time constant and TWO barriers per step instead of three (phase 4 of step s and phase 2 of
 //     step s + 1 run back to back, then phase 5 of step s and phase 3 of step s + 1);
 //   * the two roles meet at named barriers only (FULL / EMPTY per ring buffer: bar.arrive on one side, bar.sync on
 //     the other), the step warps synchronise among themselves on a 256-thread named barrier;
 //   * setmaxnreg moves registers from the draw warps (64) to the step warps (88; the fragments alone are 52 registers):
-//     256 x 88 + 128 x 64 = the 384 x 80 the CTA is launched with.
+//     256 x 88 + 128 x 64 = the 384 x 80 the CTA is launched with.  Not kept: 96 / 48 -- two side-by-side blocks
+//     need about 64 registers, the draw loop spills at 48 and the launch took 5 % longer (H100 SXM, 700 W); the
+//     step warps still spill two fragment doubles at 96.  (Budgets are multiples of 8, so 92 / 56 does not exist.)
 // Draw events, ticks and arithmetic are those of rwalk_mma_kernel (the step factor is the same expression); delta^T P
 // delta is summed as 2 delta^T U delta (below), so results agree with rwalk_mma_kernel to round-off.
 // =====================================================================================
@@ -322,9 +328,14 @@ struct MmaWsLayout {
     static constexpr int O_Y = O_X + 2 * RING;                           // axes @ z (chain-major), two buffers (slot parity)
     static constexpr int O_Q = O_Y + 2 * CH * YS;                        // partial quadratic forms per step warp
     static constexpr int O_F = O_Q + 8 * CH;                             // step factors, two rings
-    static constexpr int O_SS = O_F + 2 * DEPTH * CH;                    // |z|^2 per ring slot (draw warps' scratch)
-    static constexpr int O_LG = O_SS + DEPTH * CH;                       // log U of the radius per ring slot
-    static constexpr int O_ST = O_LG + DEPTH * CH;                       // chain state: ucur, uprop, vcur, vprop
+    // draw warps' scratch: per warp, one row per item of a buffer (DEPTH * CH / NDW of them) with the |z|^2 share of
+    // each pair block and log U of the radius block; row stride (nb + 1) | 1 <= SRMAX (odd: the one-lane-per-item
+    // reads of a column are bank-conflict free)
+    static constexpr int NBMAX = ((4 * KT < 62 ? 4 * KT : 62) + 1) / 2;  // pair blocks at the largest n of this KT
+    static constexpr int SRMAX = (NBMAX + 1) | 1;
+    static constexpr int SCW = DEPTH * CH / NDW * SRMAX;
+    static constexpr int O_SC = O_F + 2 * DEPTH * CH;
+    static constexpr int O_ST = O_SC + NDW * SCW;                        // chain state: ucur, uprop, vcur, vprop
     static constexpr int TOTAL = O_ST + CH * 4 * RS;                     // doubles
 };
 // Static schedule of the symmetric quadratic form (largest n of a KT: S = SMAX slabs): the tiles (slab s, k-tile k)
@@ -427,6 +438,8 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
         asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
         const int dw = warp - L::NSW;
         const double inv_n = 1.0 / (double)n;
+        const int nb1 = ((n + 1) >> 1) + 1;                       // Philox blocks per item: pair blocks + the radius block
+        const int SR = nb1 | 1, osc = L::O_SC + dw * L::SCW;
         for (int g0 = 0; g0 < cd.y; g0 += CH) {
             const int nlc = (cd.y - g0) < CH ? (cd.y - g0) : CH;
             for (int blk = 0; blk < NB; blk++) {
@@ -435,43 +448,49 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
                 const int nit = nd * nlc;
                 const int oXb = L::O_X + b * DB * XB;
                 if (blk >= RB) nbar_sync(BAR_EMPTY + b, 384);     // the step warps have finished with this buffer
-                for (int w = dw; w < nit; w += 2 * L::NDW) {      // two items side by side (their chains interleave)
-                    const int w2 = w + L::NDW;
-                    const bool two = w2 < nit;
-                    int sa, ca, sb, cb;
-                    if (nlc == CH) { sa = w >> 3; ca = w & 7; sb = w2 >> 3; cb = w2 & 7; }
-                    else { sa = w / nlc; ca = w - sa * nlc; sb = w2 / nlc; cb = w2 - sb * nlc; }
-                    if (!two) { sb = sa; cb = ca; }
+                // this warp's items: w = dw + NDW * k, k < cnt.  Their blocks form one flat space, task t = k * nb1 + j,
+                // dealt one block per lane, two tasks (t, t + 32) side by side while both halves are busy
+                const int cnt = (nit - dw + L::NDW - 1) / L::NDW, T = cnt * nb1;
+                auto task = [&](int t, ChainRng& g, int& j, int& off, int& o) {
+                    const int k = t / nb1, w = dw + L::NDW * k;
+                    j = t - k * nb1;
+                    int s, c2;
+                    if (nlc == CH) { s = w >> 3; c2 = w & 7; }
+                    else { s = w / nlc; c2 = w - s * nlc; }
+                    g.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + c2]);
+                    g.tick = 2u * (uint32_t)(step0 + s);
+                    off = oXb + s * XB + c2 * XS;
+                    o = osc + k * SR + j;
+                };
+                int t0 = 0;
+                for (; t0 + 32 < T; t0 += 64) {
+                    const int tb = t0 + 32 + lane;
+                    const bool two = tb < T;
                     ChainRng ga, gb;
-                    ga.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + ca]);
-                    gb.init(p.seed, chain0_ + (uint64_t)p.order[cd.x + g0 + cb]);
-                    ga.tick = 2u * (uint32_t)(step0 + sa);
-                    gb.tick = 2u * (uint32_t)(step0 + sb);
-                    double ssa, lga, ssb, lgb;
-                    ball_draw_fast(ga, oXb + sa * XB + ca * XS, true, n, lane, ssa, lga);
-                    ball_draw_fast(gb, oXb + sb * XB + cb * XS, two, n, lane, ssb, lgb);
-                    if (lane == 0) {
-                        b2n_sm[L::O_SS + sa * CH + ca] = ssa;
-                        b2n_sm[L::O_LG + sa * CH + ca] = lga;
-                        if (two) {
-                            b2n_sm[L::O_SS + sb * CH + cb] = ssb;
-                            b2n_sm[L::O_LG + sb * CH + cb] = lgb;
-                        }
-                    }
+                    int ja, offa, oa, jb, offb, ob;
+                    task(t0 + lane, ga, ja, offa, oa);
+                    task(two ? tb : t0 + lane, gb, jb, offb, ob);
+                    ball_block_fast(ga, ja, n, offa, oa, true);
+                    ball_block_fast(gb, jb, n, offb, ob, two);
+                }
+                if (t0 < T) {
+                    const bool one = t0 + lane < T;
+                    ChainRng g;
+                    int j, off, o;
+                    task(one ? t0 + lane : t0, g, j, off, o);
+                    ball_block_fast(g, j, n, off, o, one);
                 }
                 __syncwarp();
-                {   // step factors of this warp's items, one lane per item: item w = dw + NDW * lane
+                if (lane < cnt) {         // step factors, one lane per item (cnt <= DB * CH / NDW = 16)
                     const int w = dw + L::NDW * lane;
-                    if (lane < 2 * DB && w < nit) {
-                        int sa, ca;
-                        if (nlc == CH) { sa = w >> 3; ca = w & 7; }
-                        else { sa = w / nlc; ca = w - sa * nlc; }
-                        const int e = sa * CH + ca;
-                        b2n_sm[L::O_F + b * DB * CH + e] =
-                            scale_ * b2n_div(exp(b2n_sm[L::O_LG + e] * inv_n), b2n_sqrt(b2n_sm[L::O_SS + e]));
-                    }
+                    int s, c2;
+                    if (nlc == CH) { s = w >> 3; c2 = w & 7; }
+                    else { s = w / nlc; c2 = w - s * nlc; }
+                    const int o = osc + lane * SR;
+                    const double ss = ss_butterfly<1>(o, nb1 - 1, 0);
+                    b2n_sm[L::O_F + b * DB * CH + s * CH + c2] = scale_ * b2n_div(exp(b2n_sm[o + nb1 - 1] * inv_n), b2n_sqrt(ss));
                 }
-                __syncwarp();             // lane 0 rewrites the scratch in the next buffer's first pass (racecheck, r2t)
+                __syncwarp();             // the next buffer's blocks rewrite the scratch
                 __threadfence_block();
                 nbar_arrive(BAR_FULL + b, 384);
             }
