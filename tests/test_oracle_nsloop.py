@@ -188,3 +188,83 @@ def test_replicas_plumbing(fake_ops):
     summ = replicas.summarize(outs, wall)
     assert summ['replicas'] == 3 and summ['ncall'] == sum(o['ncall'] for o in outs)
     assert abs(summ['logz_mean'] - 3 * (-np.log(20.))) < 1.0
+
+
+# ---- the one-CTA limits of the device rounds (tests/test_gpu_ns_limits.py) ---------------------------------------
+def test_quadrature_past_1024_matches_mpmath():
+    """The oracle's ln X and logZ over rounds of K > 1024 against a 50-digit restatement of the same quadrature:
+    the j-th removal of round r has ln X = r ln((N-K+1)/(N+1)) + ln((N-j)/(N+1)) and the trapezoid weight
+    (L_j + L_{j-1}) / 2 X / (N - j)."""
+    import mpmath as mp
+    mp.mp.dps = 50
+    om = OL.gauss_corr(3, 0.4, 5.0)
+    N, K, R = 2500, 1100, 4
+    rng = np.random.default_rng(21)
+    u = rng.random((40 * N, 3))
+    u = u[np.argsort(om.loglike(om.prior_transform(u)))[:N]]          # the low tail: prior draws clear it at once
+    v = om.prior_transform(u)
+    l = np.array([float(om.loglike(x)) for x in v])
+    o = nsloop.BatchNS(om, u, v, l, K, 'rwalk', 1, 9, ncall=N, dlogz=0.0, unit_cube_phase=True,
+                       first_min_ncall=1 << 62)
+    for _ in range(R):
+        assert o.step()
+    _, _, dl, dlv, _ = o.dead_arrays()
+    logx, z, lprev = mp.mpf(0), mp.mpf(0), mp.mpf(0)               # exp(loglstar = -1e300) = 0
+    for r in range(R):
+        for j in range(K):
+            lx = logx + mp.log(mp.mpf(N - j) / (N + 1))
+            assert abs(float(lx) - dlv[r * K + j]) <= 1e-13
+            el = mp.exp(mp.mpf(float(dl[r * K + j])))
+            z += (el + lprev) / 2 * mp.exp(lx) / (N - j)
+            lprev = el
+        logx += mp.log(mp.mpf(N - K + 1) / (N + 1))
+    assert o.logz == pytest.approx(float(mp.log(z)), rel=1e-12)
+    assert o.logvol == pytest.approx(float(logx), rel=0, abs=1e-13)
+
+
+def test_ns_limits_case_table_reaches_every_limit():
+    """The case table of tests/test_gpu_ns_limits.py, derived with the host's shared-memory formulas on an H100's
+    227 KB opt-in limit, reaches every place where a loop of the one-CTA kernels changes form."""
+    from oracle import nslimits as NL
+    optin, T = NL.H100_SMEM_OPTIN, NL.THREADS
+    W = NL.WIDTH_CASES
+    assert {2, 3, 1025, 2048, 2049, 4097, 16384} <= {N for N, _ in W}
+    assert {1, 1023, 1024, 1025, 2048, 2049, 4097, 8192} <= {K for _, K in W}
+    lim = [NL.limits(N, K) for N, K in W]
+    assert all(NL.sort_accepts(N, optin) and NL.run_accepts(N, K, 3, 1, optin) for N, K in W)
+    assert {1, 2, 4, 8} <= {x['sort_passes'] for x in lim}
+    assert any(x['sort_padding'] == 0 and x['sort_passes'] > 1 for x in lim)
+    assert any(x['sort_padding'] > 0 and x['sort_passes'] > 1 for x in lim)
+    assert any(x['sort_padding'] == 1 for x in lim) and any(x['one_survivor'] for x in lim)
+    halves = {x['merge_half'] for x in lim}
+    assert min(halves) < T and T in halves and max(halves) > T and max(x['merge_passes'] for x in lim) >= 4
+    assert max(x['loop_passes'] for x in lim) >= 8
+    R = NL.RWALK_CASES
+    assert any(K > T and e == 1 for _, K, e in R) and any(K > T and e > 1 for _, K, e in R)
+    assert any(e > K for _, K, e in R)
+    for t in (256, 512):
+        ks = [K for tt, _, _, K in NL.THREAD_CASES if tt == t]
+        assert any(K > T for K in ks) and any(300 <= K < T for K in ks)
+        assert all(NL.limits(N, K, t)['loop_passes'] > 1 for tt, _, N, K in NL.THREAD_CASES if tt == t)
+    # the refusals: the sort's last nlive, and the bands of refused batches at that nlive
+    assert NL.sort_limit(optin) == 16384 and not NL.sort_accepts(16385, optin)
+    assert NL.refused_bands(16384, 3, 1, optin) == [(4097, 5381), (8193, 13573)]
+    assert NL.refused_bands(8192, 3, 1, optin) == []
+
+
+def test_quantized_gauss_numpy_form():
+    """oracle.nslimits.QuantizedGauss against its defining formula floor(q L_g) / q, L_g = -0.5 |v|^2."""
+    from oracle import nslimits as NL
+    rng = np.random.default_rng(4)
+    u = rng.random((400, 3))
+    for q in (4.0, 65536.0):
+        m = NL.QuantizedGauss(3, q)
+        v = m.prior_transform(u)
+        assert np.array_equal(v, -2.0 + 4.0 * u)
+        l = m.loglike(v)
+        want = [math.floor(q * (-0.5 * (x[0] * x[0] + x[1] * x[1] + x[2] * x[2]))) / q for x in v]
+        assert np.array_equal(l, want) and float(m.loglike(v[0])) == want[0]
+        assert np.all(l <= -0.5 * np.sum(v * v, axis=1)) and np.all(np.floor(l * q) == l * q)
+        t = q * (-0.5 * np.sum(v * v, axis=1))
+        assert m.min_frac == pytest.approx(np.min(np.abs(t - np.rint(t))), rel=0, abs=0)
+    assert len(np.unique(NL.QuantizedGauss(3).loglike(v))) <= 25                  # q = 4: few levels, many ties
