@@ -107,6 +107,9 @@ SYMBOLS = {
     'b2n_friends_overlap': (C.c_int, [_P, _P, _L, _I, _P]),
     'b2n_friends_unif_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _P, _P, _P, _P, _P, _P]),
     'b2n_jitter_runs': (C.c_int, [_P, _P, _P, _L, _P, _D, _I, _I, _U64, _U64, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'b2n_weighted_stats': (C.c_int, [_P, _P, _L, _I, _P, _I, _P, _P, _I, _P, _P, _P]),
+    'b2n_jitter_posterior': (C.c_int, [_P, _P, _P, _L, _P, _D, _I, _I, _U64, _U64, _P, _I, _P, _I, _P, _P, _P, _P, _P,
+                                       _P, _P]),
     'b2n_bound_set': (C.c_int, [_P, _I, _I, _P, _P, _P, _P]),
     'b2n_rwalk_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _P, _P, _P, _P, _P, _P]),
     'b2n_rslice_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _I, _P, _P, _P, _P, _P, _P, _P]),
@@ -137,6 +140,8 @@ SYMBOLS = {
     'b2n_ns_set_live_it': (C.c_int, [_P, _P]),
     'b2n_ns_get_live_it': (C.c_int, [_P, _P]),
     'b2n_resample_runs': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _P, _P, _P, _P]),
+    'b2n_resample_posterior': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _I, _P, _I,
+                                         _P, _P, _P, _P, _P, _P, _P]),
     'b2n_merge_runs': (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 

@@ -57,6 +57,8 @@ struct JArgs {
     double* out_logz; double* out_logzerr; double* out_h; double* out_kld;                // R each, may be NULL
     double* f_logvol; double* f_logwt; double* f_logz; double* f_kld;                     // R x N, may be NULL
     double* f_h; double* f_logzvar;                      // N, may be NULL (b2n_integrate_lnt only)
+    double* f_w;             // N x R (sample-major): w = exp(logwt - logz[-1]) (jitter_weights_kernel only)
+    double* s_w2;            // R x nseg: segment sums of w^2 (jitter_weights_kernel only)
 };
 
 __device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
@@ -148,9 +150,10 @@ __device__ void segment_lnt(const JArgs& A, const JSeg& s, int r, double* lt, do
 }
 
 // GIVEN: ln t read from A.lnt (b2n_integrate_lnt); the full h / logzvar arrays are written only in that mode, so the
-// instantiations of b2n_jitter_runs compile to the code they had before it existed.
-template <int PASS, bool GIVEN>
-__global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
+// instantiations of b2n_jitter_runs compile to the code they had before it existed.  WOUT (pass 2 only): also the
+// weights f_w and the segment sums of their squares s_w2 (b2n_jitter_posterior), likewise only in that mode.
+template <int PASS, bool GIVEN, bool WOUT>
+__device__ __forceinline__ void jitter_pass(const JArgs& A) {
     __shared__ double lt[JT_TILE], pv[JT_TILE], cap[JT_TILE + 1], buf[JT_CHUNK], wsum[32];
     const int64_t sg = blockIdx.x;
     const int r = blockIdx.y;
@@ -190,11 +193,11 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     // samples t + u * blockDim)
     constexpr int U = JT_TILE / JT_BLOCK;
     double* sa = buf + JT_TILE;
-    double c_r[U], k_r[U];
+    double c_r[U], k_r[U], w2_r[U];
 #pragma unroll
     for (int u = 0; u < U; u++) {
         const int i = threadIdx.x + u * JT_BLOCK;
-        c_r[u] = k_r[u] = 0.0;
+        c_r[u] = k_r[u] = w2_r[u] = 0.0;
         if (i >= L) continue;
         const int64_t j = s.a + i;
         const double l = A.logl[j], lprev = j > 0 ? A.logl[j - 1] : -1e300;
@@ -206,6 +209,11 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
         if (!GIVEN && A.wref) {             // (no KL divergence against given ln t)
             const double lp1 = cap[i] - zmax;
             k_r[u] = exp(lp1) * (lp1 - (A.wref[j] - A.zref));
+        }
+        if (WOUT) {
+            const double w = exp(cap[i] - zmax);
+            A.f_w[(size_t)j * A.R + r] = w;
+            w2_r[u] = w * w;
         }
     }
     __syncthreads();
@@ -219,11 +227,16 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     for (int u = 0; u < U; u++) {
         const int i = threadIdx.x + u * JT_BLOCK;
         if (i < L) { lt[i] = c_r[u]; pv[i] = k_r[u]; }
+        if (WOUT && i < L) cap[i] = w2_r[u];
     }
     __syncthreads();
     const double Asum = block_scan(sa, L, wsum, OpSum());
     const double Csum = block_scan(lt, L, wsum, OpSum());
     const double Ksum = block_scan(pv, L, wsum, OpSum());
+    if (WOUT) {
+        const double W2sum = block_scan(cap, L, wsum, OpSum());
+        if (threadIdx.x == 0) A.s_w2[so] = W2sum;
+    }
     if (A.f_kld)
         for (int i = threadIdx.x; i < L; i += blockDim.x) A.f_kld[fo + i] = pv[i];
     if (GIVEN) {
@@ -236,6 +249,12 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) {
     }
     if (threadIdx.x == 0) { A.sA[so] = Asum; A.sC[so] = Csum; A.sK[so] = Ksum; }
 }
+
+template <int PASS, bool GIVEN>
+__global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) { jitter_pass<PASS, GIVEN, false>(A); }
+
+// Pass 2 of b2n_jitter_posterior: jitter_pass_kernel<2, false> plus the weights.
+__global__ void __launch_bounds__(JT_BLOCK) jitter_weights_kernel(JArgs A) { jitter_pass<2, false, true>(A); }
 
 // One realisation per block: running scans over its segments in chunks of JT_TILE.
 // PASS 1: logvol (sV) and logz (sZ) before every segment, zend = logz[-1].
@@ -330,6 +349,7 @@ int jitter_launch(b2n_ctx* ctx, const JArgs& A, bool given) {
     jitter_scan_kernel<1><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     if (given) jitter_pass_kernel<2, true><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else if (A.f_w) jitter_weights_kernel<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
     else jitter_pass_kernel<2, false><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     jitter_scan_kernel<2><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
@@ -341,13 +361,14 @@ int jitter_launch(b2n_ctx* ctx, const JArgs& A, bool given) {
     return B2N_OK;
 }
 
-// Per-(realisation, segment) scratch: 7 x R x nseg, + logz[-1] per realisation.
-int jitter_scratch(b2n_ctx* ctx, JArgs& A) {
+// Per-(realisation, segment) scratch: 7 x R x nseg (8 with the w^2 sums), + logz[-1] per realisation.
+int jitter_scratch(b2n_ctx* ctx, JArgs& A, bool w2 = false) {
     const size_t rs = (size_t)A.R * A.nseg;
-    B2N_CUDA(ctx, ctx->scratch1.ensure((7 * rs + A.R) * sizeof(double)));
+    B2N_CUDA(ctx, ctx->scratch1.ensure(((w2 ? 8 : 7) * rs + A.R) * sizeof(double)));
     double* sp = ctx->scratch1.as<double>();
     A.sD = sp; A.sE = sp + rs; A.sV = sp + 2 * rs; A.sZ = sp + 3 * rs;
     A.sA = sp + 4 * rs; A.sC = sp + 5 * rs; A.sK = sp + 6 * rs; A.zend = sp + 7 * rs;
+    if (w2) A.s_w2 = sp + 7 * rs + A.R;
     return B2N_OK;
 }
 
@@ -392,14 +413,9 @@ int jitter_plan(const int64_t* n, int64_t N, int approx, std::vector<JSeg>& seg,
     return B2N_OK;
 }
 
-}  // namespace
-
-extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
-                               const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
-                               uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
-                               double* logvol_full, double* logwt_full, double* logz_full, double* kld_full) {
-    if (!ctx || !logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
-    if (!logwt_ref && (kld || kld_full)) return B2N_ERR_ARG;
+// The inputs of b2n_jitter_runs staged into A (plan, records, scratch); the output pointers are left NULL.
+int jitter_setup(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
+                 double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, bool w2, JArgs& A) {
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     std::vector<JSeg> seg;
     std::vector<int32_t> aux;
@@ -409,7 +425,6 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     const int64_t nseg = (int64_t)seg.size();
     if (nseg > INT32_MAX) return B2N_ERR_ARG;
 
-    JArgs A;
     memset(&A, 0, sizeof(A));
     const void* p;
     B2N_TRY(b2n_in(ctx, ctx->in0, logl, (size_t)N * sizeof(double), &p));
@@ -423,7 +438,19 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
     A.seg = (const JSeg*)p;
     A.N = N; A.nseg = nseg; A.R = R; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0;
-    B2N_TRY(jitter_scratch(ctx, A));
+    return jitter_scratch(ctx, A, w2);
+}
+
+}  // namespace
+
+extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
+                               const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
+                               uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
+                               double* logvol_full, double* logwt_full, double* logz_full, double* kld_full) {
+    if (!ctx || !logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
+    if (!logwt_ref && (kld || kld_full)) return B2N_ERR_ARG;
+    JArgs A;
+    B2N_TRY(jitter_setup(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, false, A));
     void* d;
     double* const sum_user[4] = {logz, logzerr, h, kld};
     double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
@@ -447,6 +474,20 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
     for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, full_user[k], *full_dev[k], (size_t)R * N * sizeof(double)));
     return b2n_finish(ctx);
+}
+
+int b2n_jitter_weights(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
+                       const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
+                       uint64_t chain0, double* const sum[4], double* w, double** w2, int64_t* nw2,
+                       const double** wref) {
+    JArgs A;
+    B2N_TRY(jitter_setup(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, true, A));
+    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
+    A.f_w = w;
+    *w2 = A.s_w2;
+    *nw2 = A.nseg;
+    *wref = A.wref;
+    return jitter_launch(ctx, A, false);
 }
 
 // compute_integrals (utils.py:1411-1467) of one record whose ln t per sample is given: logvol = cumsum(lnt), then the

@@ -14,6 +14,7 @@
 // Nothing R x N is stored; a realisation never reads another's data, so it does not depend on R.
 #include "b2n_device.cuh"
 
+#include <algorithm>
 #include <math.h>
 
 namespace {
@@ -36,6 +37,10 @@ struct RArgs {
     uint64_t seed, chain0;
     int32_t* mult;               // R x S
     double *out_logz, *out_logzerr, *out_h, *out_kld;
+    int R;
+    double* w;                   // N x R (sample-major): W = sum over a sample's copies of exp(logwt - logz[-1]),
+                                 // -0.0 for a sample not drawn (resample_weights_kernel only)
+    double* w2;                  // R: sum over the copies of exp(logwt - logz[-1])^2 (resample_weights_kernel only)
 };
 
 __device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
@@ -117,13 +122,17 @@ __device__ __forceinline__ double copy_dlv(double n, int k, bool is_end) {
     return log(c / (c + 1.0));
 }
 
-__global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) {
+// WOUT: also the weights w / w2 (b2n_resample_posterior); resample_scan_kernel, without them, compiles to the code it
+// had before they existed.
+template <bool WOUT>
+__device__ __forceinline__ void resample_scan(const RArgs& A) {
     __shared__ double xc[RS_TILE], xp[RS_TILE], xv[RS_TILE], xz[RS_TILE], wsum[32];
     const int r = blockIdx.x;
     const int32_t* m = A.mult + (size_t)r * A.S;
     const double ln_half = -0.69314718055994530942;
     double zmax = 0.0;
     double sA = 0.0, sC = 0.0, sK = 0.0;                        // sweep 2: sums of a, dh * dlogvol, KL terms
+    double sW2 = 0.0;                                           // sweep 2 (WOUT): sum of w^2 over the copies
     for (int sweep = 1; sweep <= 2; sweep++) {
         double c_cnt = 0.0, c_prev = -1.0, c_lv = 0.0, c_z = -INFINITY;   // carries across tiles
         for (int64_t t0 = 0; t0 < A.N; t0 += RS_TILE) {
@@ -177,11 +186,13 @@ __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) {
             __syncthreads();
             const double tz = block_scan(xz, L, wsum, OpLae());
             if (sweep == 2) {
-                double a_t = 0.0, c_t = 0.0, k_t = 0.0;
+                double a_t = 0.0, c_t = 0.0, k_t = 0.0, w2_t = 0.0;
                 for (int q = threadIdx.x; q < L; q += blockDim.x) {
                     const int64_t i = t0 + q;
                     const int mi = m[A.strand[i]];
+                    if (WOUT && mi == 0) A.w[(size_t)i * A.R + r] = -0.0;
                     if (mi == 0) continue;
+                    double W = 0.0;
                     const bool ie = A.end && A.end[i];
                     const double n = c_cnt + xc[q];
                     const double pidx = fmax(c_prev, q > 0 ? xp[q - 1] : -1.0);
@@ -203,10 +214,16 @@ __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) {
                             const double lp1 = w - zmax;
                             k_t += exp(lp1) * (lp1 - lp2);
                         }
+                        if (WOUT) {
+                            const double wc = exp(w - zmax);
+                            W += wc;
+                            w2_t += wc * wc;
+                        }
                         z = zn;
                         lv += d;
                         lp = l;
                     }
+                    if (WOUT) A.w[(size_t)i * A.R + r] = W;
                 }
                 // block sums (fixed association: one value per thread, then block_scan's order)
                 __syncthreads();
@@ -215,6 +232,11 @@ __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) {
                 sA += block_scan(xc, RS_BLOCK, wsum, OpSum());
                 sC += block_scan(xp, RS_BLOCK, wsum, OpSum());
                 sK += block_scan(xv, RS_BLOCK, wsum, OpSum());
+                if (WOUT) {
+                    xc[threadIdx.x] = w2_t;
+                    __syncthreads();
+                    sW2 += block_scan(xc, RS_BLOCK, wsum, OpSum());
+                }
             }
             c_cnt += tc;
             c_prev = fmax(c_prev, tp);
@@ -229,17 +251,17 @@ __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) {
     if (A.out_logzerr) A.out_logzerr[r] = sqrt(fabs(sC));       // logzvar = |cumsum(dh * dlogvol)|
     if (A.out_h) A.out_h[r] = sA - zmax;                        // h1[-1] - zmax * exp(logz[-1] - zmax)
     if (A.out_kld) A.out_kld[r] = sK;
+    if (WOUT) A.w2[r] = sW2;
 }
 
-}  // namespace
+__global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) { resample_scan<false>(A); }
+__global__ void __launch_bounds__(RS_BLOCK) resample_weights_kernel(RArgs A) { resample_scan<true>(A); }
 
-extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
-                                 const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand,
-                                 const uint8_t* end, const double* logwt_ref, double logz_ref, int32_t R,
-                                 uint64_t seed, uint64_t chain0, double* logz, double* logzerr, double* h,
-                                 double* kld, int32_t* mult) {
-    if (!ctx || !logl || !strand || !base || !piece_ptr || N < 1 || S < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
-    if (!logwt_ref && kld) return B2N_ERR_ARG;
+// The inputs of b2n_resample_runs staged into A, its multiplicities in `mult` (device, R x S) or in scratch1 (NULL),
+// followed there by R doubles for the w^2 sums when w2 is set; the output pointers are left NULL.
+int resample_setup(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S, const uint8_t* base,
+                   const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end, const double* logwt_ref,
+                   double logz_ref, int32_t R, uint64_t seed, uint64_t chain0, int32_t* mult, bool w2, RArgs& A) {
     if (piece_ptr[0] != 0 || piece_ptr[N] < 0 || (piece_ptr[N] > 0 && !piece_strand)) return B2N_ERR_ARG;
     for (int64_t i = 0; i < N; i++)
         if (strand[i] < 0 || strand[i] >= S || piece_ptr[i + 1] < piece_ptr[i]) return B2N_ERR_ARG;
@@ -253,7 +275,6 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
     if (nbase == 0) return b2n_fail(ctx, B2N_ERR_ARG, "b2n_resample_runs: the record has no base strand");
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
 
-    RArgs A;
     memset(&A, 0, sizeof(A));
     const void* p;
     B2N_TRY(b2n_in(ctx, ctx->in0, logl, (size_t)N * sizeof(double), &p));
@@ -270,16 +291,53 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
     A.end = (const uint8_t*)p;
     B2N_TRY(b2n_in_host(ctx, ctx->scratch3, ids.data(), ids.size() * sizeof(int32_t), &p));
     A.base_ids = (const int32_t*)p;
-    A.N = N; A.S = S; A.nbase = nbase; A.nadd = nadd; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0;
+    A.N = N; A.S = S; A.nbase = nbase; A.nadd = nadd; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0; A.R = R;
+    const size_t msz = (size_t)R * S * sizeof(int32_t), mpad = (msz + 255) / 256 * 256;
+    if (mult) {
+        A.mult = mult;
+        if (w2) {
+            B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)R * sizeof(double)));
+            A.w2 = ctx->scratch1.as<double>();
+        }
+    } else {
+        B2N_CUDA(ctx, ctx->scratch1.ensure(w2 ? mpad + (size_t)R * sizeof(double) : msz));
+        A.mult = ctx->scratch1.as<int32_t>();
+        if (w2) A.w2 = (double*)((char*)ctx->scratch1.p + mpad);
+    }
+    return B2N_OK;
+}
+
+// The two launches on the stream (the multiplicities zeroed first); pass 2 with the weights when A.w is set.
+int resample_launch(b2n_ctx* ctx, const RArgs& A, int32_t R) {
+    B2N_CUDA(ctx, cudaMemsetAsync(A.mult, 0, (size_t)R * A.S * sizeof(int32_t), ctx->stream));
+    const dim3 grid((unsigned)((std::max(A.nbase, A.nadd) + RS_BLOCK - 1) / RS_BLOCK), (unsigned)R);
+    resample_mult_kernel<<<grid, RS_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    if (A.w) resample_weights_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
+    else resample_scan_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
+    B2N_LAUNCH_CHECK(ctx);
+    return B2N_OK;
+}
+
+}  // namespace
+
+extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                                 const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand,
+                                 const uint8_t* end, const double* logwt_ref, double logz_ref, int32_t R,
+                                 uint64_t seed, uint64_t chain0, double* logz, double* logzerr, double* h,
+                                 double* kld, int32_t* mult) {
+    if (!ctx || !logl || !strand || !base || !piece_ptr || N < 1 || S < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
+    if (!logwt_ref && kld) return B2N_ERR_ARG;
     void* d;
     const size_t msz = (size_t)R * S * sizeof(int32_t);
+    int32_t* dmult = nullptr;
     if (mult) {
         B2N_TRY(b2n_out(ctx, ctx->out4, mult, msz, &d));
-    } else {
-        B2N_CUDA(ctx, ctx->scratch1.ensure(msz));
-        d = ctx->scratch1.p;
+        dmult = (int32_t*)d;
     }
-    A.mult = (int32_t*)d;
+    RArgs A;
+    B2N_TRY(resample_setup(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R, seed,
+                           chain0, dmult, false, A));
     double* const sum_user[4] = {logz, logzerr, h, kld};
     double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
     DevBuf* const sum_buf[4] = {&ctx->out0, &ctx->out1, &ctx->out2, &ctx->out3};
@@ -289,15 +347,24 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
     }
 
     B2N_TIME_BEGIN(ctx);
-    B2N_CUDA(ctx, cudaMemsetAsync(A.mult, 0, msz, ctx->stream));
-    const dim3 grid((unsigned)((std::max(nbase, nadd) + RS_BLOCK - 1) / RS_BLOCK), (unsigned)R);
-    resample_mult_kernel<<<grid, RS_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
-    resample_scan_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
-    B2N_LAUNCH_CHECK(ctx);
+    B2N_TRY(resample_launch(ctx, A, R));
     B2N_TIME_END(ctx);
 
     B2N_TRY(b2n_out_done(ctx, mult, A.mult, msz));
     for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
     return b2n_finish(ctx);
+}
+
+int b2n_resample_weights(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                         const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
+                         const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
+                         double* const sum[4], double* w, double** w2, const double** wref) {
+    RArgs A;
+    B2N_TRY(resample_setup(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R, seed,
+                           chain0, nullptr, true, A));
+    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
+    A.w = w;
+    *w2 = A.w2;
+    *wref = A.wref;
+    return resample_launch(ctx, A, R);
 }

@@ -596,6 +596,109 @@ def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, cha
     return o
 
 
+# ---- posterior summaries (include/b200nest.h, b2n_weighted_stats / b2n_jitter_posterior / b2n_resample_posterior) --
+def _post_outputs(R, n, q, moments):
+    o = dict(mean=np.empty((R, n)), cov=np.empty((R, n, n))) if moments else {}
+    if q is not None:
+        o['quantiles'] = np.empty((R, n, len(q)))
+    return o
+
+
+def _post_q(q):
+    if q is None:
+        return None
+    q = f64(np.atleast_1d(q))
+    if q.ndim != 1 or len(q) < 1:
+        raise ValueError("q must be a non-empty list of quantiles")
+    if np.any(q < 0.0) or np.any(q > 1.0) or np.isnan(q).any():
+        raise ValueError("Quantiles must be between 0. and 1.")
+    return q
+
+
+def _post_x(x, N):
+    x = f64(x)
+    if x.ndim != 2 or len(x) != N or x.shape[1] < 1:
+        raise ValueError("the sample positions must be an array of shape (%d, ndim)" % N)
+    return x
+
+
+def weighted_stats(x, w, shift, q=None, moments=True, ctx=None):
+    """Weighted means, covariances and quantiles of the samples x (N x n) under R weight vectors w (R x N, >= 0),
+    second moments about `shift` (n).  Returns dict(mean (R x n), cov (R x n x n)) with moments=True and
+    quantiles (R x n x nq) with q."""
+    ctx = _ctx(ctx)
+    w = f64(np.atleast_2d(w))
+    R, N = w.shape
+    x = _post_x(x, N)
+    n = x.shape[1]
+    shift = f64(shift)
+    if shift.shape != (n,):
+        raise ValueError("shift must hold one number per dimension")
+    q = _post_q(q)
+    o = _post_outputs(R, n, q, moments)
+    ctx.check(ctx.lib.b2n_weighted_stats(ctx.h, ptr(x), N, n, ptr(w), R, ptr(shift), ptr(q),
+                                         0 if q is None else len(q), ptr(o.get('mean')), ptr(o.get('cov')),
+                                         ptr(o.get('quantiles'))))
+    return o
+
+
+def jitter_posterior(logl, samples_n, x, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, q=None,
+                     ctx=None):
+    """jitter_runs plus, per realisation, the weighted mean (R x n), covariance (R x n x n) and, with q, quantiles
+    (R x n x nq) of the sample positions x (N x n).  logwt_ref / logz_ref (the record's own) are required."""
+    ctx = _ctx(ctx)
+    logl = f64(logl)
+    n_ = np.ascontiguousarray(samples_n, dtype=np.int64)
+    N, R = len(logl), int(R)
+    if len(n_) != N:
+        raise ValueError("logl and samples_n differ in length")
+    wref = f64(logwt_ref)
+    if len(wref) != N:
+        raise ValueError("logwt_ref and logl differ in length")
+    x = _post_x(x, N)
+    q = _post_q(q)
+    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R), kld=np.empty(R))
+    o.update(_post_outputs(R, x.shape[1], q, True))
+    ctx.check(ctx.lib.b2n_jitter_posterior(ctx.h, ptr(logl), ptr(n_), N, ptr(wref), float(logz_ref),
+                                           int(bool(approx)), R, int(seed), int(chain0), ptr(x), x.shape[1], ptr(q),
+                                           0 if q is None else len(q), ptr(o['logz']), ptr(o['logzerr']), ptr(o['h']),
+                                           ptr(o['kld']), ptr(o['mean']), ptr(o['cov']), ptr(o.get('quantiles'))))
+    return o
+
+
+def resample_posterior(logl, strand, base, piece_ptr, piece_strand, end, x, R, seed, chain0=0, logwt_ref=None,
+                       logz_ref=None, q=None, ctx=None):
+    """resample_runs plus, per realisation, the weighted mean, covariance and, with q, quantiles of the sample
+    positions x (N x n) over the realisation's copies.  logwt_ref / logz_ref (the record's own) are required."""
+    ctx = _ctx(ctx)
+    logl = f64(logl)
+    N = len(logl)
+    strand = np.ascontiguousarray(strand, dtype=np.int32)
+    base = np.ascontiguousarray(base, dtype=np.uint8)
+    pp = np.ascontiguousarray(piece_ptr, dtype=np.int64)
+    ps = np.ascontiguousarray(piece_strand, dtype=np.int32)
+    if len(strand) != N or len(pp) != N + 1:
+        raise ValueError("logl, strand and piece_ptr differ in length")
+    if end is not None:
+        end = np.ascontiguousarray(end, dtype=np.uint8)
+        if len(end) != N:
+            raise ValueError("logl and end differ in length")
+    S, R = len(base), int(R)
+    wref = f64(logwt_ref)
+    if len(wref) != N:
+        raise ValueError("logwt_ref and logl differ in length")
+    x = _post_x(x, N)
+    q = _post_q(q)
+    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R), kld=np.empty(R))
+    o.update(_post_outputs(R, x.shape[1], q, True))
+    ctx.check(ctx.lib.b2n_resample_posterior(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps),
+                                             ptr(end), ptr(wref), float(logz_ref), R, int(seed), int(chain0), ptr(x),
+                                             x.shape[1], ptr(q), 0 if q is None else len(q), ptr(o['logz']),
+                                             ptr(o['logzerr']), ptr(o['h']), ptr(o['kld']), ptr(o['mean']),
+                                             ptr(o['cov']), ptr(o.get('quantiles'))))
+    return o
+
+
 def merge_runs(logl, samples_n, run_ptr, nbase, lowedge=None, arrays=True, ctx=None):
     """R records merged into one (merge_runs / _merge_two, utils.py:1817-1900, 2045-2225; include/b200nest.h,
     b2n_merge_runs).  logl / samples_n: the records concatenated, run r = [run_ptr[r], run_ptr[r + 1]), each run's

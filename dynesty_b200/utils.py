@@ -6,8 +6,12 @@ What is mirrored (reference py/dynesty/utils.py, same names / meaning):
   unravel_run   :1711-1814   a run split into its strands
   kld_error     :1932-1997   the KL divergence from the run to such a realisation
   merge_runs    :1817-1929   several runs merged into one (``b2n_merge_runs``)
+  mean_and_cov  :1081-1117   weighted mean and covariance (``b2n_weighted_stats``)
+  quantile      :1196-1233   weighted quantiles (``b2n_weighted_stats``; unweighted: np.percentile)
 and the batched forms the dynamic sampler's stopping function needs: ``jitter_realisations`` (``b2n_jitter_runs``) and
-``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches.
+``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches,
+and ``posterior_realisations``: the same realisations with the posterior mean, covariance and quantiles of each
+(``b2n_jitter_posterior`` / ``b2n_resample_posterior``).
 
 Randomness: realisation r of a call is the B2N Philox stream (seed, chain0 + r) (include/b200nest.h), so a (seed,
 chain) pair names one realisation: it is the same whether it is computed alone or in a batch of any size.
@@ -237,6 +241,70 @@ def unravel_run(res):
             r['batch_bounds'] = res['batch_bounds']
         out.append(r)
     return out
+
+
+# ---------------------------------------------------------------------------------------------- posterior summaries
+def mean_and_cov(samples, weights, ctx=None):
+    """mean_and_cov (utils.py:1081-1117): the weighted mean (ndim) and covariance (ndim x ndim) of samples (nsamples x
+    ndim), cov = wsum / (wsum^2 - w2sum) sum w (x - mean)(x - mean)^T.  weights may also be R x nsamples: then R
+    weight vectors at once, returning (R x ndim, R x ndim x ndim).  Computed on the GPU in FP64 (b2n_weighted_stats),
+    second moments about the mean under the summed weights."""
+    x = np.ascontiguousarray(samples, dtype=np.float64)
+    w = np.asarray(weights, dtype=np.float64)
+    if x.ndim != 2:
+        raise ValueError("samples must be an array of shape (nsamples, ndim)")
+    if w.ndim not in (1, 2) or w.shape[-1] != len(x):
+        raise ValueError("Dimension mismatch: the weights must have shape (nsamples,) or (R, nsamples).")
+    wt = np.atleast_2d(w).sum(axis=0)
+    shift = wt @ x / wt.sum() if wt.sum() > 0 else x.mean(axis=0)
+    o = ops.weighted_stats(x, np.atleast_2d(w), shift, ctx=ctx)
+    return (o['mean'][0], o['cov'][0]) if w.ndim == 1 else (o['mean'], o['cov'])
+
+
+def quantile(x, q, weights=None, ctx=None):
+    """quantile (utils.py:1196-1233): the weighted quantiles q of the samples x, as a list (np.interp's rule on the
+    cdf of the sorted samples, include/b200nest.h b2n_weighted_stats; computed on the GPU); without weights,
+    np.percentile(x, 100 q), as the reference does."""
+    x = np.atleast_1d(x)
+    q = np.atleast_1d(q)
+    if np.any(q < 0.0) or np.any(q > 1.0):
+        raise ValueError("Quantiles must be between 0. and 1.")
+    if weights is None:
+        return np.percentile(x, list(100.0 * q))
+    weights = np.atleast_1d(weights)
+    if len(x) != len(weights):
+        raise ValueError("Dimension mismatch: len(weights) != len(x).")
+    x = np.asarray(x, dtype=np.float64).reshape(-1, 1)
+    o = ops.weighted_stats(x, np.asarray(weights, dtype=np.float64)[None, :], x.mean(axis=0), q=q, moments=False,
+                           ctx=ctx)
+    return o['quantiles'][0, 0].tolist()
+
+
+def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=False, q=None, ctx=None):
+    """n_mc realisations of `res` -- jitter_run's (error='jitter') or resample_run's (error='resample') -- with the
+    posterior summaries of each over res['samples'].  Returns the dict of jitter_realisations / resample_realisations
+    (logz, logzerr, h, kld; n_mc values each) plus mean (n_mc x ndim), cov (n_mc x ndim x ndim) and, with q,
+    quantiles (n_mc x ndim x nq): mean_and_cov / quantile of each realisation's samples and weights
+    exp(logwt - logz[-1]), a resampled point's copies counted each.  Realisation r is the stream (seed, chain0 + r):
+    the one jitter_run(res, seed, chain0 + r) / resample_run(res, seed, chain0 + r) returns."""
+    if error not in ('jitter', 'resample'):
+        raise ValueError("Input `'error'` option '{}' is not valid.".format(error))
+    logl = np.asarray(res['logl'], dtype=float)
+    x = np.asarray(res['samples']) if 'samples' in res else np.empty((0, 0))
+    if x.ndim != 2 or len(x) != len(logl) or x.shape[1] < 1:
+        raise ValueError("posterior_realisations needs the sample positions of every point (res['samples']); "
+                         "a run made with keep_samples=False has none")
+    logz_ref = float(np.asarray(res['logz'])[-1])
+    if error == 'jitter':
+        return ops.jitter_posterior(logl, samples_n_of(res), x, int(n_mc), int(seed), chain0=int(chain0),
+                                    approx=approx, logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx)
+    plan = strand_plan(res)
+    if not plan['base'].any():
+        raise ValueError("The provided `Results` does not include any points initially sampled from the prior!")
+    pptr, pstr = _piece_csr(logl, plan)
+    return ops.resample_posterior(logl, plan['strand'], plan['base'], pptr, pstr, plan['end'], x, int(n_mc),
+                                  int(seed), chain0=int(chain0), logwt_ref=res['logwt'], logz_ref=logz_ref, q=q,
+                                  ctx=ctx)
 
 
 # ---------------------------------------------------------------------------------------------- merging runs

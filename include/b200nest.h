@@ -362,6 +362,49 @@ int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, i
                       const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
                       double* logz, double* logzerr, double* h, double* kld, int32_t* mult);
 
+/* ---- posterior summaries of weighted sample sets (utils.py:1081-1117 mean_and_cov, :1196-1233 quantile) ----------
+ * R weight vectors over one set of N samples x (N x n, row-major).  For each realisation r (DESIGN.md section 15.3):
+ *   mean_r = sum_i w_ri x_i / wsum,  cov_r = wsum / (wsum^2 - w2sum) sum_i w_ri (x_i - mean_r)(x_i - mean_r)^T,
+ * wsum = sum_i w_ri and w2sum = sum of the squares of the weights (of the copies, on the resample path).  The second
+ * moments are accumulated about a shift c (n) that is the same for every realisation of a call, then corrected:
+ * sum w (x - mean)(x - mean)^T = sum w (x - c)(x - c)^T - wsum (mean - c)(mean - c)^T.
+ * quant_r[j][t]: the weighted quantile q[t] of coordinate j.  Nodes: the samples present in realisation r, sorted
+ * stably by (x_ij, i); a node carries its weight (on the resample path, the sum over the sample's copies).  Node k has
+ * cdf C_k = sum_{l<k} w_l / sum_{l<M-1} w_l (M nodes, so the last node's own weight never enters); for q, take p = the
+ * largest k with C_k <= q: the result is x_p if q == C_p or p is the last node, else the linear interpolation from
+ * (C_p, x_p) towards (C_{p+1}, x_{p+1}) -- np.interp's rule with repeated cdf values.  A node of weight 0 is a node; a
+ * weight of -0.0 (the sign bit set) marks a sample ABSENT from the realisation.  A set whose sum_{l<M-1} w_l is 0 (one
+ * node, or all the weight on the last node) gives NaN; with one sample present wsum^2 == w2sum and cov is undefined,
+ * as in the reference.  q must lie in [0, 1]; 1 <= n <= 1024, N * n < 2^31.
+ * All FP64.  Sums over N are split in pieces whose bounds depend on N only and reduced in a fixed order, without float
+ * atomics: the same bits every call, and realisation r's outputs do not depend on R or on the other realisations.
+ * Outputs, each may be NULL: mean (R x n), cov (R x n x n), quant (R x n x nq), row-major.  A fixed number of kernel
+ * launches (plus those of one CUB segmented radix sort of the n coordinates when quant is asked for), whatever R, N or
+ * n; R <= 65535.  Synchronises in host-pointer mode.
+ *
+ * b2n_weighted_stats: the weights given, w (R x N, >= 0), and the shift given, shift (n); x, w, shift, q host or device
+ * like the other arrays of the call. */
+int b2n_weighted_stats(b2n_ctx* ctx, const double* x, int64_t N, int32_t n, const double* w, int32_t R,
+                       const double* shift, const double* q, int32_t nq, double* mean, double* cov, double* quant);
+
+/* b2n_jitter_posterior / b2n_resample_posterior: the realisations of b2n_jitter_runs / b2n_resample_runs (same
+ * arguments, streams and summaries logz, logzerr, h, kld -- bit for bit), together with the posterior summaries above of
+ * each realisation over the record's sample positions x (N x n, in record order):
+ *   jitter     w_ri = exp(logwt_ri - logz_r[-1]), every sample present;
+ *   resample   W_ri = the sum over sample i's copies of exp(logwt_copy - logz_r[-1]), w2sum over the copies; a sample
+ *              drawn 0 times is absent.
+ * logwt_ref is required: the shift is the record's own weighted mean, sum exp(logwt_ref) x / sum exp(logwt_ref),
+ * computed on the device.  The weights stay on the device (an N x R buffer). */
+int b2n_jitter_posterior(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
+                         const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
+                         uint64_t chain0, const double* x, int32_t n, const double* q, int32_t nq, double* logz,
+                         double* logzerr, double* h, double* kld, double* mean, double* cov, double* quant);
+int b2n_resample_posterior(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                           const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand,
+                           const uint8_t* end, const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed,
+                           uint64_t chain0, const double* x, int32_t n, const double* q, int32_t nq, double* logz,
+                           double* logzerr, double* h, double* kld, double* mean, double* cov, double* quant);
+
 /* ---- merge_runs (utils.py:1817-1900, _merge_two :2045-2225 of the reference) ---------------------------------------
  * R dead-point records of N samples in all, concatenated: run r is samples [run_ptr[r], run_ptr[r + 1]), its logl
  * ascending and free of NaN (assumed, not checked), samples_n its live count at every sample (>= 1).  The first nbase
