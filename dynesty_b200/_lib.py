@@ -100,6 +100,8 @@ SYMBOLS = {
     'b2n_moments': (C.c_int, [_P, _P, _L, _I, _P, _P]),
     'b2n_improve_covar': (C.c_int, [_P, _P, _I, _P, _P, _P, _P, _P]),
     'b2n_fp64_peak': (C.c_int, [_P, _I, _I, C.POINTER(_D), C.POINTER(_D)]),
+    'b2n_fp64_latency': (C.c_int, [_P, _I, _I, C.POINTER(_D)]),
+    'b2n_dmma_probe': (C.c_int, [_P, _I, _P, _P, _P, _P]),
     'b2n_scale_to_logvol': (C.c_int, [_P, _I, _I, _P, _P, _P, _P, _P, _P]),
     'b2n_bootstrap_expand': (C.c_int, [_P, _P, _L, _I, _I, _I, _U64, _U64, _P]),
     'b2n_friends_update': (C.c_int, [_P, _P, _L, _I, _I, _I, _P, _I, _U64, _U64, _P, _P, _P, _P, _P, _P, _P]),

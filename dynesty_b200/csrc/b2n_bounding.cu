@@ -1170,27 +1170,47 @@ extern "C" int b2n_improve_covar(b2n_ctx* ctx, const double* covar, int32_t n, d
 }
 
 // ------------------------------------------------------------------ FP64 issue ceilings (bench.py roofline)
-// What the chain kernels are made of is FP64 FMA (vector pipe) and FP64 m8n8k4 MMA (tensor pipe, DMMA).  Both
-// ceilings are MEASURED here instead of quoted: every warp runs `iters` rounds of 16 independent dependency
-// chains (DFMA: 16 accumulators per thread; DMMA: 8 accumulator pairs per warp), 8 warps x 8 CTAs per SM.
-__global__ void __launch_bounds__(256) fp64_peak_kernel(int kind, int iters, double seed, double* __restrict__ out) {
+// What the chain kernels are made of is FP64 FMA (vector pipe) and FP64 MMA (tensor pipe, DMMA).  Both ceilings are
+// MEASURED here instead of quoted: every warp runs `iters` rounds of 16 independent dependency chains (DFMA: 16
+// accumulators per thread; m8n8k4: 8 accumulator pairs per warp; the m16n8 shapes: 4 accumulator quads per warp),
+// 8 warps x 8 CTAs per SM.  KIND: 0 DFMA, 1 m8n8k4, 2 m16n8k4, 3 m16n8k8, 4 m16n8k16 (bench.py reports against 0, 1).
+template <int KIND>
+__device__ __forceinline__ void fp64_op(double* acc, double a, double b) {
+    if constexpr (KIND == 0) {
+        acc[0] = fma(acc[0], a, b);
+    } else if constexpr (KIND == 1) {
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
+                     : "+d"(acc[0]), "+d"(acc[1])
+                     : "d"(a), "d"(b));
+    } else if constexpr (KIND == 2) {
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                     : "+d"(acc[0]), "+d"(acc[1]), "+d"(acc[2]), "+d"(acc[3])
+                     : "d"(a), "d"(a), "d"(b));
+    } else if constexpr (KIND == 3) {
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                     "{%0,%1,%2,%3};\n"
+                     : "+d"(acc[0]), "+d"(acc[1]), "+d"(acc[2]), "+d"(acc[3])
+                     : "d"(a), "d"(a), "d"(a), "d"(a), "d"(b), "d"(b));
+    } else {
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+                     : "+d"(acc[0]), "+d"(acc[1]), "+d"(acc[2]), "+d"(acc[3])
+                     : "d"(a), "d"(a), "d"(a), "d"(a), "d"(a), "d"(a), "d"(a), "d"(a), "d"(b), "d"(b), "d"(b), "d"(b));
+    }
+}
+// accumulator doubles per lane of one instruction, flop per instruction (DFMA: per lane; MMA: per warp)
+__host__ __device__ constexpr int fp64_acc(int kind) { return kind == 0 ? 1 : (kind == 1 ? 2 : 4); }
+static double fp64_flop(int kind) { return kind == 0 ? 2.0 : 2.0 * (kind == 1 ? 8 : 16) * 8 * (kind <= 2 ? 4 : (kind == 3 ? 8 : 16)); }
+
+template <int KIND>
+__global__ void __launch_bounds__(256) fp64_peak_kernel(int iters, double seed, double* __restrict__ out) {
     double acc[16];
 #pragma unroll
     for (int i = 0; i < 16; i++) acc[i] = seed * (double)(threadIdx.x + i + 1);
     const double a = 1.0 + 1e-9 * seed, b = 1e-9 * (double)(threadIdx.x & 3);
-    if (kind == 0) {
-        for (int it = 0; it < iters; it++) {
+    for (int it = 0; it < iters; it++) {
 #pragma unroll
-            for (int i = 0; i < 16; i++) acc[i] = fma(acc[i], a, b);
-        }
-    } else {
-        for (int it = 0; it < iters; it++) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 2)
-                asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                             : "+d"(acc[i]), "+d"(acc[i + 1])
-                             : "d"(a), "d"(b));
-        }
+        for (int i = 0; i < 16; i += fp64_acc(KIND)) fp64_op<KIND>(&acc[i], a, b);
     }
     double s = 0.0;
 #pragma unroll
@@ -1198,8 +1218,28 @@ __global__ void __launch_bounds__(256) fp64_peak_kernel(int kind, int iters, dou
     if (s == 123456.789) out[blockIdx.x * blockDim.x + threadIdx.x] = s;     // keeps the chains alive
 }
 
+// Dependent-issue latency: ONE warp, ONE dependency chain of `iters` instructions, timed in SM clocks.
+template <int KIND>
+__global__ void __launch_bounds__(32) fp64_latency_kernel(int iters, double seed, long long* __restrict__ cyc,
+                                                          double* __restrict__ out) {
+    double acc[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) acc[i] = seed * (double)(threadIdx.x + i + 1);
+    const double a = 1.0 + 1e-9 * seed, b = 1e-9 * (double)(threadIdx.x & 3);
+    __syncwarp();
+    const long long t0 = clock64();
+    for (int it = 0; it < iters; it++) fp64_op<KIND>(acc, a, b);
+    const long long t1 = clock64();
+    const double s = acc[0] + acc[1] + acc[2] + acc[3];
+    if (threadIdx.x == 0) cyc[0] = t1 - t0;
+    if (s == 123456.789) out[threadIdx.x] = s;
+}
+
+#define B2N_FP64_KIND(K_, CALL) \
+    switch (K_) { case 0: CALL(0); break; case 1: CALL(1); break; case 2: CALL(2); break; case 3: CALL(3); break; default: CALL(4); break; }
+
 extern "C" int b2n_fp64_peak(b2n_ctx* ctx, int32_t kind, int32_t iters, double* tflops, double* ms_out) {
-    if (!ctx || (kind != 0 && kind != 1) || iters < 1 || !tflops) return B2N_ERR_ARG;
+    if (!ctx || kind < 0 || kind > 4 || iters < 1 || !tflops) return B2N_ERR_ARG;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     const int ctas = ctx->sm_count * 8, threads = 256;
     B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)ctas * threads * sizeof(double)));
@@ -1210,7 +1250,9 @@ extern "C" int b2n_fp64_peak(b2n_ctx* ctx, int32_t kind, int32_t iters, double* 
     float best = 1e30f;
     for (int rep = 0; rep < 5; rep++) {          // rep 0 warms up; best of the rest
         cudaEventRecord(e0, st);
-        fp64_peak_kernel<<<ctas, threads, 0, st>>>(kind, iters, 1.0 + rep, ctx->scratch1.as<double>());
+#define B2N_PEAK(K) fp64_peak_kernel<K><<<ctas, threads, 0, st>>>(iters, 1.0 + rep, ctx->scratch1.as<double>())
+        B2N_FP64_KIND(kind, B2N_PEAK)
+#undef B2N_PEAK
         cudaEventRecord(e1, st);
         ctx->launches++;
         B2N_CUDA(ctx, cudaEventSynchronize(e1));
@@ -1221,12 +1263,97 @@ extern "C" int b2n_fp64_peak(b2n_ctx* ctx, int32_t kind, int32_t iters, double* 
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     B2N_CUDA(ctx, cudaGetLastError());
-    // flop count: DFMA = 2 flop per lane per instruction; DMMA m8n8k4 = 2*8*8*4 = 512 flop per warp instruction
-    const double per_thread_instr = (double)iters * (kind == 0 ? 16.0 : 8.0);
-    const double flops = kind == 0 ? per_thread_instr * 2.0 * (double)ctas * threads
-                                   : per_thread_instr * 512.0 * (double)ctas * (threads / 32);
+    // flop: DFMA 2 per lane per instruction; DMMA m x n x k: 2 m n k per warp instruction (m8n8k4: 512)
+    const double per_thread_instr = (double)iters * (16.0 / fp64_acc(kind));
+    const double flops = kind == 0 ? per_thread_instr * fp64_flop(0) * (double)ctas * threads
+                                   : per_thread_instr * fp64_flop(kind) * (double)ctas * (threads / 32);
     *tflops = flops / ((double)best * 1e-3) / 1e12;
     if (ms_out) *ms_out = (double)best;
+    return B2N_OK;
+}
+
+extern "C" int b2n_fp64_latency(b2n_ctx* ctx, int32_t kind, int32_t iters, double* cycles) {
+    if (!ctx || kind < 0 || kind > 4 || iters < 1 || !cycles) return B2N_ERR_ARG;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    B2N_CUDA(ctx, ctx->scratch1.ensure(32 * sizeof(double) + sizeof(long long)));
+    double* out = ctx->scratch1.as<double>();
+    long long* cyc = reinterpret_cast<long long*>(out + 32);
+    cudaStream_t st = ctx->stream;
+    double best = 1e30;
+    for (int rep = 0; rep < 5; rep++) {          // rep 0 warms up; best of the rest
+#define B2N_LAT(K) fp64_latency_kernel<K><<<1, 32, 0, st>>>(iters, 1.0 + rep, cyc, out)
+        B2N_FP64_KIND(kind, B2N_LAT)
+#undef B2N_LAT
+        ctx->launches++;
+        B2N_CUDA(ctx, cudaGetLastError());
+        long long c = 0;
+        B2N_CUDA(ctx, b2n_copy_sync(ctx, &c, cyc, sizeof(c), cudaMemcpyDeviceToHost));
+        if (rep > 0 && (double)c < best) best = (double)c;
+    }
+    *cycles = best / (double)iters;
+    return B2N_OK;
+}
+#undef B2N_FP64_KIND
+
+// Bit-identity probe of the FP64 MMA shapes: one warp per 16 x 8 tile, A 16 x 8, B 8 x 8 (k x n), C 16 x 8, all
+// row-major.  out[4][tile][16 x 8]:
+//   0  m16n8k4 (k 0..3) + C
+//   1  two m8n8k4 (rows 0..7, rows 8..15; k 0..3) + C
+//   2  m16n8k8 (k 0..7) + C
+//   3  two chained m16n8k4 (k 0..3, then k 4..7) + C
+// Fragments (PTX ISA, mma .f64): g = lane / 4, t = lane % 4; A rows g / g + 8, column t (+ 4 for the k 4..7 half);
+// B row t (+ 4), column g; C / D rows g / g + 8, columns 2 t, 2 t + 1.
+__global__ void __launch_bounds__(32) dmma_probe_kernel(const double* __restrict__ A, const double* __restrict__ B,
+                                                        const double* __restrict__ Cm, double* __restrict__ out, int ntiles) {
+    const int tile = blockIdx.x, lane = threadIdx.x, g = lane >> 2, t = lane & 3;
+    const double* a = A + (size_t)tile * 128;
+    const double* b = B + (size_t)tile * 64;
+    const double* c = Cm + (size_t)tile * 128;
+    const double a00 = a[g * 8 + t], a10 = a[(g + 8) * 8 + t], a01 = a[g * 8 + t + 4], a11 = a[(g + 8) * 8 + t + 4];
+    const double b0 = b[t * 8 + g], b1 = b[(t + 4) * 8 + g];
+    const double c0 = c[g * 8 + 2 * t], c1 = c[g * 8 + 2 * t + 1], c2 = c[(g + 8) * 8 + 2 * t], c3 = c[(g + 8) * 8 + 2 * t + 1];
+    double r[4][4];
+    r[0][0] = c0; r[0][1] = c1; r[0][2] = c2; r[0][3] = c3;
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(r[0][0]), "+d"(r[0][1]), "+d"(r[0][2]), "+d"(r[0][3]) : "d"(a00), "d"(a10), "d"(b0));
+    r[1][0] = c0; r[1][1] = c1; r[1][2] = c2; r[1][3] = c3;
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
+                 : "+d"(r[1][0]), "+d"(r[1][1]) : "d"(a00), "d"(b0));
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
+                 : "+d"(r[1][2]), "+d"(r[1][3]) : "d"(a10), "d"(b0));
+    r[2][0] = c0; r[2][1] = c1; r[2][2] = c2; r[2][3] = c3;
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                 : "+d"(r[2][0]), "+d"(r[2][1]), "+d"(r[2][2]), "+d"(r[2][3])
+                 : "d"(a00), "d"(a10), "d"(a01), "d"(a11), "d"(b0), "d"(b1));
+    r[3][0] = c0; r[3][1] = c1; r[3][2] = c2; r[3][3] = c3;
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(r[3][0]), "+d"(r[3][1]), "+d"(r[3][2]), "+d"(r[3][3]) : "d"(a00), "d"(a10), "d"(b0));
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(r[3][0]), "+d"(r[3][1]), "+d"(r[3][2]), "+d"(r[3][3]) : "d"(a01), "d"(a11), "d"(b1));
+#pragma unroll
+    for (int o = 0; o < 4; o++) {
+        double* d = out + ((size_t)o * ntiles + tile) * 128;
+        d[g * 8 + 2 * t] = r[o][0];
+        d[g * 8 + 2 * t + 1] = r[o][1];
+        d[(g + 8) * 8 + 2 * t] = r[o][2];
+        d[(g + 8) * 8 + 2 * t + 1] = r[o][3];
+    }
+}
+
+extern "C" int b2n_dmma_probe(b2n_ctx* ctx, int32_t ntiles, const double* a, const double* b, const double* c,
+                              double* out) {
+    if (!ctx || ntiles < 1 || !a || !b || !c || !out) return B2N_ERR_ARG;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    const void *da, *db, *dc;
+    B2N_TRY(b2n_in_host(ctx, ctx->in0, a, (size_t)ntiles * 128 * sizeof(double), &da));
+    B2N_TRY(b2n_in_host(ctx, ctx->in1, b, (size_t)ntiles * 64 * sizeof(double), &db));
+    B2N_TRY(b2n_in_host(ctx, ctx->in2, c, (size_t)ntiles * 128 * sizeof(double), &dc));
+    const size_t ob = (size_t)4 * ntiles * 128 * sizeof(double);
+    B2N_CUDA(ctx, ctx->out0.ensure(ob));
+    dmma_probe_kernel<<<ntiles, 32, 0, ctx->stream>>>((const double*)da, (const double*)db, (const double*)dc,
+                                                      ctx->out0.as<double>(), ntiles);
+    B2N_LAUNCH_CHECK(ctx);
+    B2N_CUDA(ctx, b2n_copy_sync(ctx, out, ctx->out0.p, ob, cudaMemcpyDeviceToHost));
     return B2N_OK;
 }
 

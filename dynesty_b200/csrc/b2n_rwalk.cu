@@ -52,6 +52,13 @@ __device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double
                  : "+d"(d0), "+d"(d1)
                  : "d"(a), "d"(b));
 }
+// Two m8n8k4 stacked: a0 / d[0..1] are rows g of the first 8-row half, a1 / d[2..3] rows g of the second, b shared.
+// One DMMA.16x8x4 gives the bits of the two DMMA.8x8x4 (tests/test_gpu_mmaws_golden.py, scripts/dmma_shapes.py).
+__device__ __forceinline__ void dmma1684(double (&d)[4], double a0, double a1, double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+                 : "d"(a0), "d"(a1), "d"(b));
+}
 
 // Shared-memory plan of rwalk_mma_kernel, in doubles: the kernel takes its offsets from it, the host its size.
 // KT = k-tiles of 4 columns (n <= 4*KT); CH = chains in lock-step per CTA (8 -> 256 threads, two
@@ -302,6 +309,10 @@ __global__ void __launch_bounds__(256, 2) rwalk_mma_kernel(const RwalkParams p) 
 //   * warps 0..7 run the step phases of rwalk_mma_kernel on register-resident DMMA fragments, with every shared-memory
 //     offset a compile-time constant and TWO barriers per step instead of three (phase 4 of step s and phase 2 of
 //     step s + 1 run back to back, then phase 5 of step s and phase 3 of step s + 1);
+//   * the direction product axes @ z (phase 2) runs on DMMA.16x8x4, two slabs per instruction, dealt over all 8 step
+//     warps as (slab pair, k-tile parity) items: at KT = 13 a warp issues at most 7 DMMAs per step instead of 13, 52
+//     per CTA-step instead of 91.  Each parity is summed in the order of the former per-slab accumulator pair and
+//     phase 3 adds the two halves, so the chains keep their bits;
 //   * the two roles meet at named barriers only (FULL / EMPTY per ring buffer: bar.arrive on one side, bar.sync on
 //     the other), the step warps synchronise among themselves on a 256-thread named barrier;
 //   * setmaxnreg moves registers from the draw warps (64) to the step warps (88; the fragments alone are 52 registers):
@@ -502,17 +513,22 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
     } else {
         // =============================== step warps ===============================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 88;");
-        const int S = (n + 7) >> 3;
-        const int s_it = warp;                                    // slab of this warp's item of axes @ z
-        const bool has_item = warp < S;
-        double fragA[KT];
+        // axes @ z: item (slab pair pp, k-tile parity kpar) -- the rows of slabs 2 pp, 2 pp + 1 as the two halves of
+        // m16n8k4 tiles, over the k-tiles of one parity.  The even items sum the even k-tiles in order, the odd items
+        // the odd ones, and phase 3 adds the two: the association of the former per-slab accumulator pair (d, e).
+        constexpr int NP = (L::SMAX + 1) / 2;                      // slab pairs (KT = 13: slab 7 of pair 3 is padding)
+        constexpr int NKH = (KT + 1) / 2;                          // k-tiles of the even parity; the odd one has KT / 2
+        const bool has_item = warp < 2 * NP;
+        const int pp = warp % NP, kpar = warp / NP;               // the two parities of a pair on different schedulers
+        double fragA[2 * NKH];                                    // k-tile 2 j + kpar: [2 j] slab 2 pp, [2 j + 1] slab 2 pp + 1
         {
             const double* Ag = p.axesT + (size_t)cd.z * n * n;
-            const int row = 8 * s_it + (lane >> 2);
+            const int row = 16 * pp + (lane >> 2);
 #pragma unroll
-            for (int kt = 0; kt < KT; kt++) {
-                const int col = 4 * kt + (lane & 3);
-                fragA[kt] = (has_item && row < n && col < n) ? Ag[(size_t)col * n + row] : 0.0;
+            for (int j = 0; j < NKH; j++) {
+                const int col = 4 * (2 * j + kpar) + (lane & 3);
+                fragA[2 * j] = (has_item && row < n && col < n) ? Ag[(size_t)col * n + row] : 0.0;
+                fragA[2 * j + 1] = (has_item && row + 8 < n && col < n) ? Ag[(size_t)col * n + row + 8] : 0.0;
             }
         }
         // The precision matrix is symmetric: delta^T P delta = 2 delta^T U delta with U = its upper triangle and HALF
@@ -523,7 +539,7 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
         B2N_WARP_SWITCH(warp, B2N_SYM_LOAD)
 #undef B2N_SYM_LOAD
         const int xb_it = (lane >> 2) * XS + (lane & 3);                          // B fragment of k-tile 0
-        const int yst_it = L::O_Y + 2 * (lane & 3) * YS + 8 * s_it + (lane >> 2);
+        const int yr_it = 16 * pp + (lane >> 2);                                  // row of d[0], d[1] (chains 2 t, 2 t + 1)
         const int xr_it = 2 * (lane & 3) * XS + (lane >> 2);                      // delta[row 0 of a slab] of chain c0
         const int pk = p.m.prior_kind;
         const int c = warp;                                       // chain slot owned by this warp
@@ -545,30 +561,38 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
             double lcur = 0.0;
             bool ok = true;
 
-            // phase 2 of a ring slot: Y[rows of slab][chains] = A_slab @ X -- the DMMAs are issued here, their result
-            // is stored by phase2_store AFTER the chain phases of the same barrier interval (the tensor pipe works on
-            // the next-but-one step while the warp walks through the latency chains of phases 5 and 3)
-            auto phase2_issue = [&](int oXs, double& d0, double& d1, double& e0, double& e1) {
-                d0 = 0.0; d1 = 0.0; e0 = 0.0; e1 = 0.0;
-                const int xb = oXs + xb_it;
+            // phase 2 of a ring slot: this warp's half of axes @ z (d) -- the DMMAs are issued in the interval before
+            // the one that stores them (phase2_store), so the tensor pipe works on the next-but-one step while the warp
+            // walks through the latency chains of phases 5 and 3, and the z rows the DMMAs read are dead by the store
+            auto phase2_issue = [&](int oXs, double (&d)[4]) {
+                d[0] = 0.0; d[1] = 0.0; d[2] = 0.0; d[3] = 0.0;
+                const int xb = oXs + xb_it + 4 * kpar;
 #pragma unroll
-                for (int kt = 0; kt + 1 < KT; kt += 2) {
-                    dmma884(d0, d1, fragA[kt], b2n_sm[xb + 4 * kt]);
-                    dmma884(e0, e1, fragA[kt + 1], b2n_sm[xb + 4 * kt + 4]);
+                for (int j = 0; j < NKH; j++)
+                    if (KT % 2 == 0 || j + 1 < NKH || kpar == 0) dmma1684(d, fragA[2 * j], fragA[2 * j + 1], b2n_sm[xb + 8 * j]);
+            };
+            // the even half goes to Y[buf], the odd half to oo (chain stride so): the z rows of its own ring slot (read by
+            // nobody once the slot's DMMAs are issued; phase 3 reads each element before it writes delta over it) or,
+            // for slot 0, Y[1].  Rows of the padding slab are not stored: they would run past a chain's row of Y.
+            auto phase2_store = [&](int buf, int oo, int so, const double (&d)[4]) {
+                const int cs = kpar ? so : YS;
+                const int o = (kpar ? oo : L::O_Y + buf * CH * YS) + 2 * (lane & 3) * cs + yr_it;
+                b2n_sm[o] = d[0];
+                b2n_sm[o + cs] = d[1];
+                if (2 * pp + 1 < L::SMAX) {
+                    b2n_sm[o + 8] = d[2];
+                    b2n_sm[o + cs + 8] = d[3];
                 }
-                if (KT & 1) dmma884(d0, d1, fragA[KT - 1], b2n_sm[xb + 4 * (KT - 1)]);
             };
-            auto phase2_store = [&](int buf, double d0, double d1, double e0, double e1) {
-                b2n_sm[yst_it + buf * CH * YS] = d0 + e0;
-                b2n_sm[yst_it + buf * CH * YS + YS] = d1 + e1;
-            };
-            auto phase3 = [&](int oXs, double fac, int oy) {   // u' = u + fac*y, wrap / reflect / cube test, prior, delta -> X[s][c]
+            // u' = u + fac*y with y = the even half at oy + the odd half at oz, wrap / reflect / cube test, prior,
+            // delta -> X[s][c]
+            auto phase3 = [&](int oXs, double fac, int oy, int oz) {
                 if (PLAIN) {
                     const int i0 = lane, i1 = lane + 32;
                     const bool v0 = i0 < n, v1 = i1 < n;
                     double t0 = 0.5, t1 = 0.5;
-                    if (v0) t0 = fma(fac, b2n_sm[oy + i0], b2n_sm[oucur + i0]);
-                    if (v1) t1 = fma(fac, b2n_sm[oy + i1], b2n_sm[oucur + i1]);
+                    if (v0) t0 = fma(fac, b2n_sm[oy + i0] + b2n_sm[oz + i0], b2n_sm[oucur + i0]);
+                    if (v1) t1 = fma(fac, b2n_sm[oy + i1] + b2n_sm[oz + i1], b2n_sm[oucur + i1]);
                     const bool good = (t0 > 0.0 && t0 < 1.0) && (t1 > 0.0 && t1 < 1.0);
                     if (v0) {
                         const double vi = fma(b2n_sm[L::O_P1 + i0], t0, b2n_sm[L::O_P0 + i0]);
@@ -587,7 +611,7 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
                 }
                 bool good = true;
                 for (int i = lane; i < n; i += 32) {
-                    double t = fma(fac, b2n_sm[oy + i], b2n_sm[oucur + i]);
+                    double t = fma(fac, b2n_sm[oy + i] + b2n_sm[oz + i], b2n_sm[oucur + i]);
                     const uint32_t f = fl[i];
                     if (f & B2N_DIM_PERIODIC) t = mod1(t);
                     if (f & B2N_DIM_REFLECTIVE) t = reflect1(t);
@@ -630,38 +654,34 @@ __global__ void __launch_bounds__(384, 2) rwalk_mmaws_kernel(const RwalkParams p
             };
 
             // Two barrier intervals per step,
-            //   I(g) = phase 4 of slot g                          C(g) = [issue phase 2 of slot g + 2] phase 5 of slot g,
-            //                                                            phase 3 of slot g + 1, [store phase 2]
-            // per ring buffer (nd <= 8 slots), with a prologue
+            //   I(g) = [store phase 2 of slot g + 1] phase 4 of slot g
+            //   C(g) = [issue phase 2 of slot g + 2] phase 5 of slot g, phase 3 of slot g + 1
+            // per ring buffer (nd <= 8 slots), with a prologue that stores slot 0 and issues slot 1
             for (int blk = 0; blk < NB; blk++) {
                 const int b = blk & 1, step0 = blk * DB;
                 const int nd = (p.walks - step0) < DB ? (p.walks - step0) : DB;
                 const int oXb = L::O_X + b * DB * XB, oFb = L::O_F + b * DB * CH;
+                double d[4];                                      // phase 2 of the next slot, issued and not yet stored
                 nbar_sync(BAR_FULL + b, 384);                     // the draw warps have filled this buffer
                 if (has_item) {
-                    double d0, d1, e0, e1;
-                    phase2_issue(oXb, d0, d1, e0, e1);
-                    phase2_store(0, d0, d1, e0, e1);
-                    if (nd > 1) {
-                        phase2_issue(oXb + XB, d0, d1, e0, e1);
-                        phase2_store(1, d0, d1, e0, e1);
-                    }
+                    phase2_issue(oXb, d);
+                    phase2_store(0, L::O_Y + CH * YS, YS, d);
+                    if (nd > 1) phase2_issue(oXb + XB, d);
                 }
                 nbar_sync(BAR_STEP, 256);
-                if (live) phase3(oXb, b2n_sm[oFb + c], L::O_Y + c * YS);
+                if (live) phase3(oXb, b2n_sm[oFb + c], L::O_Y + c * YS, L::O_Y + (CH + c) * YS);
                 nbar_sync(BAR_STEP, 256);
                 for (int s2 = 0; s2 < nd; s2++) {
+                    const int oXn = oXb + (s2 + 1) * XB;          // slot s2 + 1
+                    if (has_item && s2 + 1 < nd) phase2_store((s2 + 1) & 1, oXn, XS, d);
                     phase4(oXb + s2 * XB);
                     nbar_sync(BAR_STEP, 256);
                     // every read of this ring buffer is done: hand it back to the draw warps (if they will ask for it)
                     if (s2 == nd - 1 && blk + 2 < NB) nbar_arrive(BAR_EMPTY + b, 384);
-                    const bool p2 = has_item && s2 + 2 < nd;
-                    double d0, d1, e0, e1;
-                    if (p2) phase2_issue(oXb + (s2 + 2) * XB, d0, d1, e0, e1);
+                    if (has_item && s2 + 2 < nd) phase2_issue(oXb + (s2 + 2) * XB, d);
                     if (live) phase5();
                     if (s2 + 1 < nd) {
-                        if (live) phase3(oXb + (s2 + 1) * XB, b2n_sm[oFb + (s2 + 1) * CH + c], L::O_Y + (((s2 + 1) & 1) * CH + c) * YS);
-                        if (p2) phase2_store(s2 & 1, d0, d1, e0, e1);
+                        if (live) phase3(oXn, b2n_sm[oFb + (s2 + 1) * CH + c], L::O_Y + (((s2 + 1) & 1) * CH + c) * YS, oXn + c * XS);
                         nbar_sync(BAR_STEP, 256);
                     }
                 }

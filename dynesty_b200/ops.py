@@ -124,12 +124,38 @@ def improve_covar(covar, ctx=None):
     return bool(good.value), cov, am, axes, warn.value
 
 
+FP64_KINDS = {'fma': 0, 'mma': 1, 'mma16x8x4': 2, 'mma16x8x8': 3, 'mma16x8x16': 4}
+
+
 def fp64_peak(kind, iters=20000, ctx=None):
-    """Measured FP64 ceiling in TFLOP/s: kind 'fma' (vector pipe) or 'mma' (m8n8k4 tensor pipe)."""
+    """Measured FP64 ceiling in TFLOP/s: kind 'fma' (vector pipe), 'mma' (m8n8k4 tensor pipe) or one of the
+    m16n8 shapes 'mma16x8x4', 'mma16x8x8', 'mma16x8x16'."""
     ctx = _ctx(ctx)
     t, ms = C.c_double(0.0), C.c_double(0.0)
-    ctx.check(ctx.lib.b2n_fp64_peak(ctx.h, {'fma': 0, 'mma': 1}[kind], int(iters), C.byref(t), C.byref(ms)))
+    ctx.check(ctx.lib.b2n_fp64_peak(ctx.h, FP64_KINDS[kind], int(iters), C.byref(t), C.byref(ms)))
     return t.value, ms.value
+
+
+def fp64_latency(kind, iters=4096, ctx=None):
+    """Dependent-issue latency of fp64_peak's instruction `kind`, in SM clocks: one warp, one dependency chain."""
+    ctx = _ctx(ctx)
+    cyc = C.c_double(0.0)
+    ctx.check(ctx.lib.b2n_fp64_latency(ctx.h, FP64_KINDS[kind], int(iters), C.byref(cyc)))
+    return cyc.value
+
+
+def dmma_probe(a, b, c, ctx=None):
+    """The FP64 MMA shapes on tiles a (T, 16, 8), b (T, 8, 8) (k x n), c (T, 16, 8): a dict of (T, 16, 8) results
+    'k4' (one m16n8k4 on k 0..3), 'k4x2rows' (two m8n8k4, rows 0..7 and 8..15), 'k8' (one m16n8k8) and
+    'k4x2steps' (two chained m16n8k4, k 0..3 then 4..7), each plus c (b2n_dmma_probe)."""
+    ctx = _ctx(ctx)
+    a, b, c = (np.ascontiguousarray(x, dtype=np.float64) for x in (a, b, c))
+    T = a.shape[0]
+    if a.shape != (T, 16, 8) or b.shape != (T, 8, 8) or c.shape != (T, 16, 8):
+        raise ValueError('dmma_probe: tiles must be (T, 16, 8), (T, 8, 8), (T, 16, 8)')
+    out = np.empty((4, T, 16, 8))
+    ctx.check(ctx.lib.b2n_dmma_probe(ctx.h, T, ptr(a), ptr(b), ptr(c), ptr(out)))
+    return dict(zip(('k4', 'k4x2rows', 'k8', 'k4x2steps'), out))
 
 
 def scale_to_logvol(covs, ams, axes, axlens, logvols, targets, ctx=None):

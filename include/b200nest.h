@@ -288,9 +288,20 @@ int b2n_improve_covar(b2n_ctx* ctx, const double* covar, int32_t n, double* cov_
                       double* axes, int32_t* good, uint32_t* warn);
 
 /* Measured FP64 issue ceilings of this GPU for bench.py's roofline: kind 0 = FP64 FMA (vector pipe),
- * kind 1 = FP64 m8n8k4 MMA (tensor pipe); `iters` rounds of 16 independent chains per thread, all SMs.
+ * kind 1 = FP64 m8n8k4 MMA (tensor pipe), kinds 2, 3, 4 = the m16n8k4, m16n8k8, m16n8k16 MMA shapes;
+ * `iters` rounds of 16 independent accumulator chains per thread, all SMs.
  * *tflops, *ms (best of 4 timed launches, CUDA events): host outputs.  Synchronises. */
 int b2n_fp64_peak(b2n_ctx* ctx, int32_t kind, int32_t iters, double* tflops, double* ms);
+
+/* Dependent-issue latency of the instruction of b2n_fp64_peak's `kind`: one warp, one chain of `iters`
+ * instructions, SM clocks per instruction (best of 4 launches) in *cycles (host).  Synchronises. */
+int b2n_fp64_latency(b2n_ctx* ctx, int32_t kind, int32_t iters, double* cycles);
+
+/* Bit-identity probe of the FP64 MMA shapes on `ntiles` tiles (host arrays, row-major): a[ntiles][16][8],
+ * b[ntiles][8][8] (k x n), c[ntiles][16][8].  out[4][ntiles][16][8]: 0 = one m16n8k4 (k 0..3) + c,
+ * 1 = two m8n8k4 (rows 0..7 and 8..15, k 0..3) + c, 2 = one m16n8k8 + c, 3 = two chained m16n8k4
+ * (k 0..3, then k 4..7) + c.  Synchronises. */
+int b2n_dmma_probe(b2n_ctx* ctx, int32_t ntiles, const double* a, const double* b, const double* c, double* out);
 
 /* Ellipsoid.scale_to_logvol for K ellipsoids (bounding.py:242-276, 478-495).
  * target_logvols: host, K.  covs/ams/axes/axlens/logvols updated in place. */
