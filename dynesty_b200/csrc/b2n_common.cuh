@@ -172,6 +172,22 @@ int b2n_bound_set_dev(b2n_ctx* ctx, int K, int nc, const double* dctrs, const do
 // Device pointers; uses ctx->scratch0 / scratch1; does not synchronise.
 int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
                       double* logwt, double* logz, double* logzvar, double* h);
+// The realisations of b2n_jitter_runs (b2n_jitter.cu): the record staged, the call's timer started (B2N_TIME_BEGIN),
+// the passes enqueued; no synchronisation.  sum[4]: logz, logzerr, h, kld (R each); full: NULL or logvol, logwt, logz,
+// kld (R x N each); device pointers, each may be NULL.  With w (device, N x R), pass 2 also writes the weights
+// exp(logwt - logz[-1]) and the per-segment sums of their squares, *w2 (R x *nw2, in ctx->scratch1), and *wref is the
+// record's logwt on the device.  Uses ctx->in0..in3, scratch0 and scratch1.
+int b2n_jitter_produce(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
+                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, double* const sum[4],
+                       double* const full[4], double* w, const double** w2, int64_t* nw2, const double** wref);
+// The same for b2n_resample_runs (b2n_resample.cu): mult, the multiplicities (device, R x S), may be NULL (then they
+// live in ctx->scratch1); with w, the weights are -0.0 for a sample not drawn and *w2 holds R sums (*nw2 = 1).  Uses
+// ctx->in0..in3 and scratch0..scratch3.
+int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                         const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
+                         const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
+                         double* const sum[4], int32_t* mult, double* w, const double** w2, int64_t* nw2,
+                         const double** wref);
 
 void b2n_peer_release(b2n_ctx* ctx);
 
@@ -296,6 +312,31 @@ static inline int b2n_out_done(b2n_ctx* ctx, void* dst, const void* dev, size_t 
     B2N_CUDA(ctx, cudaMemcpyAsync(dst, dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
     return B2N_OK;
 }
+// The outputs of a run-statistics entry point (b2n_jitter.cu, b2n_resample.cu, b2n_posterior.cu, b2n_merge.cu) as
+// (caller pointer, bytes) pairs.  bind() sets dev[k], where output k is written: NULL for a NULL output, the caller's
+// pointer in device-pointer mode, else a 256-byte aligned slice of ctx->out0, which none of their producers uses.
+// done() copies the staged outputs back to the caller.
+template <int K>
+struct B2nOutStage {
+    void* user[K];
+    size_t bytes[K];
+    void* dev[K];
+    int bind(b2n_ctx* ctx) {
+        const bool host = ctx->ptr_mode != B2N_PTR_DEVICE;
+        size_t off[K], end = 0;
+        for (int k = 0; k < K; k++) {
+            off[k] = (end + 255) / 256 * 256;
+            if (user[k]) end = off[k] + bytes[k];
+        }
+        if (host && end) B2N_CUDA(ctx, ctx->out0.ensure(end));
+        for (int k = 0; k < K; k++) dev[k] = !user[k] ? nullptr : host ? ctx->out0.as<char>() + off[k] : user[k];
+        return B2N_OK;
+    }
+    int done(b2n_ctx* ctx) const {
+        for (int k = 0; k < K; k++) B2N_TRY(b2n_out_done(ctx, user[k], dev[k], bytes[k]));
+        return B2N_OK;
+    }
+};
 static inline int b2n_finish(b2n_ctx* ctx) {
     if (ctx->ptr_mode == B2N_PTR_HOST) B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2N_OK;

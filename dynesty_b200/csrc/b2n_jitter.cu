@@ -23,7 +23,12 @@
 //
 // b2n_integrate_lnt (below, for b2n_merge.cu) runs the same passes in a deterministic mode: one realisation whose ln t
 // per sample is read from an array (segment_lnt<true>), over a plan of tick-0 segments only.
+//
+// Host side: b2n_jitter_produce stages a record and enqueues the passes, for b2n_jitter_runs (below) and for
+// b2n_jitter_posterior (b2n_posterior.cu, with the weights of pass 2); the entry points stage their outputs through
+// B2nOutStage (b2n_common.cuh).  The block scan and its operators are b2n_scan.cuh's.
 #include "b2n_device.cuh"
+#include "b2n_scan.cuh"
 
 #include <algorithm>
 #include <math.h>
@@ -60,58 +65,6 @@ struct JArgs {
     double* f_w;             // N x R (sample-major): w = exp(logwt - logz[-1]) (jitter_weights_kernel only)
     double* s_w2;            // R x nseg: segment sums of w^2 (jitter_weights_kernel only)
 };
-
-__device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
-    if (a == -INFINITY) return b;
-    if (b == -INFINITY) return a;
-    const double m = fmax(a, b);
-    return m + log1p(exp(-fabs(a - b)));
-}
-struct OpSum {
-    __device__ static double id() { return 0.0; }
-    __device__ double operator()(double a, double b) const { return a + b; }
-};
-struct OpLae {
-    __device__ static double id() { return -INFINITY; }
-    __device__ double operator()(double a, double b) const { return lae(a, b); }
-};
-
-// In-place inclusive scan of x[0, n) (shared memory, n <= 8 * blockDim) with a fixed association: thread t owns a
-// contiguous run, then warp shuffles, then the warp totals.  Returns the total (identity for n == 0) to every thread.
-template <class Op>
-__device__ double block_scan(double* x, int n, double* wsum, Op op) {
-    const int t = threadIdx.x, lane = t & 31, w = t >> 5, nw = blockDim.x >> 5;
-    const int ipt = (n + blockDim.x - 1) / blockDim.x;
-    const int i0 = min(t * ipt, n), i1 = min(i0 + ipt, n);
-    double acc = Op::id();
-    for (int i = i0; i < i1; i++) { acc = op(acc, x[i]); x[i] = acc; }
-    double v = acc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const double u = __shfl_up_sync(B2N_FULL, v, o);
-        if (lane >= o) v = op(u, v);
-    }
-    if (lane == 31) wsum[w] = v;
-    __syncthreads();
-    if (w == 0) {
-        double s = lane < nw ? wsum[lane] : Op::id();
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const double u = __shfl_up_sync(B2N_FULL, s, o);
-            if (lane >= o) s = op(u, s);
-        }
-        if (lane < nw) wsum[lane] = s;
-    }
-    __syncthreads();
-    double ex = __shfl_up_sync(B2N_FULL, v, 1);
-    if (lane == 0) ex = Op::id();
-    if (w > 0) ex = op(wsum[w - 1], ex);
-    if (t > 0)
-        for (int i = i0; i < i1; i++) x[i] = op(ex, x[i]);
-    const double total = wsum[nw - 1];
-    __syncthreads();
-    return total;
-}
 
 // ln t of the segment's samples into lt[0, len)
 template <bool GIVEN>
@@ -413,10 +366,11 @@ int jitter_plan(const int64_t* n, int64_t N, int approx, std::vector<JSeg>& seg,
     return B2N_OK;
 }
 
-// The inputs of b2n_jitter_runs staged into A (plan, records, scratch); the output pointers are left NULL.
-int jitter_setup(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
-                 double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, bool w2, JArgs& A) {
-    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+}  // namespace
+
+int b2n_jitter_produce(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
+                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, double* const sum[4],
+                       double* const full[4], double* w, const double** w2, int64_t* nw2, const double** wref) {
     std::vector<JSeg> seg;
     std::vector<int32_t> aux;
     B2N_TRY(jitter_plan(samples_n, N, approx, seg, aux));
@@ -425,6 +379,7 @@ int jitter_setup(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int
     const int64_t nseg = (int64_t)seg.size();
     if (nseg > INT32_MAX) return B2N_ERR_ARG;
 
+    JArgs A;
     memset(&A, 0, sizeof(A));
     const void* p;
     B2N_TRY(b2n_in(ctx, ctx->in0, logl, (size_t)N * sizeof(double), &p));
@@ -438,10 +393,15 @@ int jitter_setup(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int
     B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
     A.seg = (const JSeg*)p;
     A.N = N; A.nseg = nseg; A.R = R; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0;
-    return jitter_scratch(ctx, A, w2);
-}
+    B2N_TRY(jitter_scratch(ctx, A, w != nullptr));
+    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
+    if (full) { A.f_logvol = full[0]; A.f_logwt = full[1]; A.f_logz = full[2]; A.f_kld = full[3]; }
+    A.f_w = w;
+    if (w) { *w2 = A.s_w2; *nw2 = A.nseg; *wref = A.wref; }
 
-}  // namespace
+    B2N_TIME_BEGIN(ctx);
+    return jitter_launch(ctx, A, false);
+}
 
 extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
                                const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
@@ -449,45 +409,18 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
                                double* logvol_full, double* logwt_full, double* logz_full, double* kld_full) {
     if (!ctx || !logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
     if (!logwt_ref && (kld || kld_full)) return B2N_ERR_ARG;
-    JArgs A;
-    B2N_TRY(jitter_setup(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, false, A));
-    void* d;
-    double* const sum_user[4] = {logz, logzerr, h, kld};
-    double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
-    DevBuf* const sum_buf[4] = {&ctx->out4, &ctx->out5, &ctx->out6, &ctx->out7};
-    for (int k = 0; k < 4; k++) {
-        B2N_TRY(b2n_out(ctx, *sum_buf[k], sum_user[k], (size_t)R * sizeof(double), &d));
-        *sum_dev[k] = (double*)d;
-    }
-    double* const full_user[4] = {logvol_full, logwt_full, logz_full, kld_full};
-    double** const full_dev[4] = {&A.f_logvol, &A.f_logwt, &A.f_logz, &A.f_kld};
-    DevBuf* const full_buf[4] = {&ctx->out0, &ctx->out1, &ctx->out2, &ctx->out3};
-    for (int k = 0; k < 4; k++) {
-        B2N_TRY(b2n_out(ctx, *full_buf[k], full_user[k], (size_t)R * N * sizeof(double), &d));
-        *full_dev[k] = (double*)d;
-    }
-
-    B2N_TIME_BEGIN(ctx);
-    B2N_TRY(jitter_launch(ctx, A, false));
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    const size_t rb = (size_t)R * sizeof(double), fb = rb * N;
+    B2nOutStage<8> O{{logz, logzerr, h, kld, logvol_full, logwt_full, logz_full, kld_full},
+                     {rb, rb, rb, rb, fb, fb, fb, fb}};
+    B2N_TRY(O.bind(ctx));
+    double* d[8];
+    for (int k = 0; k < 8; k++) d[k] = (double*)O.dev[k];
+    B2N_TRY(b2n_jitter_produce(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, d, d + 4, nullptr,
+                               nullptr, nullptr, nullptr));
     B2N_TIME_END(ctx);
-
-    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
-    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, full_user[k], *full_dev[k], (size_t)R * N * sizeof(double)));
+    B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);
-}
-
-int b2n_jitter_weights(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
-                       const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
-                       uint64_t chain0, double* const sum[4], double* w, double** w2, int64_t* nw2,
-                       const double** wref) {
-    JArgs A;
-    B2N_TRY(jitter_setup(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, true, A));
-    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
-    A.f_w = w;
-    *w2 = A.s_w2;
-    *nw2 = A.nseg;
-    *wref = A.wref;
-    return jitter_launch(ctx, A, false);
 }
 
 // compute_integrals (utils.py:1411-1467) of one record whose ln t per sample is given: logvol = cumsum(lnt), then the

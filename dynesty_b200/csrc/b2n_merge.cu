@@ -14,7 +14,8 @@
 //   then the passes of b2n_jitter.cu in their deterministic mode (b2n_integrate_lnt): logvol, logwt, logz, logzvar, h.
 //
 // The node tables of every launch are built on the host from run_ptr / nbase / lowedge and uploaded once, so the
-// launches follow each other on the stream without a host round trip.
+// launches follow each other on the stream without a host round trip.  The f64 outputs are staged through
+// B2nOutStage (b2n_common.cuh); perm and samples_n are copied out of the last ping-pong buffer.
 #include "b2n_device.cuh"
 
 #include <algorithm>
@@ -182,14 +183,11 @@ extern "C" int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* s
     }
     double* d_lnt = (double*)((char*)ctx->work1.p + (size_t)N * 24);
 
-    void* d;
-    double* const fu[6] = {last3, logvol, logwt, logz, logzvar, h};
+    const size_t nb = (size_t)N * sizeof(double);
+    B2nOutStage<6> O{{last3, logvol, logwt, logz, logzvar, h}, {3 * sizeof(double), nb, nb, nb, nb, nb}};
+    B2N_TRY(O.bind(ctx));
     double* fd[6];
-    DevBuf* const fb[6] = {&ctx->out2, &ctx->out3, &ctx->out4, &ctx->out5, &ctx->out6, &ctx->out7};
-    for (int k = 0; k < 6; k++) {
-        B2N_TRY(b2n_out(ctx, *fb[k], fu[k], (k ? (size_t)N : 3) * sizeof(double), &d));
-        fd[k] = (double*)d;
-    }
+    for (int k = 0; k < 6; k++) fd[k] = (double*)O.dev[k];
 
     B2N_TIME_BEGIN(ctx);
     merge_init_kernel<<<blocks(N), MG_BLOCK, 0, ctx->stream>>>(d_logl, d_n, N, b[0], b[1]);
@@ -210,6 +208,6 @@ extern "C" int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* s
     const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (perm) B2N_CUDA(ctx, cudaMemcpyAsync(perm, m.src, (size_t)N * sizeof(int64_t), kind, ctx->stream));
     if (samples_n_out) B2N_CUDA(ctx, cudaMemcpyAsync(samples_n_out, m.n, (size_t)N * sizeof(int64_t), kind, ctx->stream));
-    for (int k = 0; k < 6; k++) B2N_TRY(b2n_out_done(ctx, fu[k], fd[k], (k ? (size_t)N : 3) * sizeof(double)));
+    B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);
 }

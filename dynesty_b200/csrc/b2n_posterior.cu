@@ -19,24 +19,15 @@
 //                                                      chunk holding the last node whose cdf is <= q
 // Every split is over N in pieces whose bounds depend on N only, every reduction runs in a fixed order and realisation
 // r reads only its own column of W: no float atomics, the same bits every call, and row r does not depend on R.
+//
+// The realisation entries take their weights from the producers b2n_jitter_produce / b2n_resample_produce
+// (b2n_common.cuh); every entry point stages its outputs (summaries, mean, cov, quantiles) through B2nOutStage.
 #include "b2n_device.cuh"
 
 #include <cub/device/device_segmented_radix_sort.cuh>
 
 #include <math.h>
 #include <vector>
-
-// The producers (b2n_jitter.cu, b2n_resample.cu): their realisations on the stream, with the summaries in sum[4]
-// (device pointers, each may be NULL), the weights in w (device, N x R) and the w^2 partials (R x nw2) in their scratch;
-// *wref: the record's logwt on the device.
-int b2n_jitter_weights(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N,
-                       const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
-                       uint64_t chain0, double* const sum[4], double* w, double** w2, int64_t* nw2,
-                       const double** wref);
-int b2n_resample_weights(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
-                         const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
-                         const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
-                         double* const sum[4], double* w, double** w2, const double** wref);
 
 namespace {
 
@@ -438,32 +429,6 @@ int post_check(int64_t N, int n, int R, const double* x, int nq, const double* q
     return B2N_OK;
 }
 
-// Caller outputs mean / cov / quant: device pointers to write (the caller's in device-pointer mode, else staging in
-// ctx->work1), and their copies back.
-struct PostOut {
-    double* user[3];
-    double* dev[3];
-    size_t bytes[3];
-    int stage(b2n_ctx* ctx, double* mean, double* cov, double* quant, int R, int n, int nq) {
-        user[0] = mean; user[1] = cov; user[2] = quant;
-        bytes[0] = (size_t)R * n * 8; bytes[1] = (size_t)R * n * n * 8; bytes[2] = (size_t)R * n * nq * 8;
-        const bool host = ctx->ptr_mode != B2N_PTR_DEVICE;
-        Bump b{nullptr};
-        for (int k = 0; k < 3; k++) if (user[k]) b.take<char>(bytes[k]);
-        if (host) B2N_CUDA(ctx, ctx->work1.ensure(b.off + 256));
-        Bump s{host ? ctx->work1.as<char>() : nullptr};
-        for (int k = 0; k < 3; k++) {
-            dev[k] = nullptr;
-            if (user[k]) dev[k] = host ? s.take<double>(bytes[k] / 8) : user[k];
-        }
-        return B2N_OK;
-    }
-    int done(b2n_ctx* ctx) {
-        for (int k = 0; k < 3; k++) B2N_TRY(b2n_out_done(ctx, user[k], dev[k], bytes[k]));
-        return B2N_OK;
-    }
-};
-
 }  // namespace
 
 extern "C" int b2n_weighted_stats(b2n_ctx* ctx, const double* x, int64_t N, int32_t n, const double* w, int32_t R,
@@ -488,9 +453,10 @@ extern "C" int b2n_weighted_stats(b2n_ctx* ctx, const double* x, int64_t N, int3
     double* Wt = ctx->work0.as<double>();
     double* w2 = Wt + (size_t)N * R;
     J.W = Wt; J.w2 = w2; J.nw2 = 1;
-    PostOut O;
-    B2N_TRY(O.stage(ctx, mean, cov, quant, R, n, nq));
-    J.mean = O.dev[0]; J.cov = O.dev[1]; J.quant = O.dev[2];
+    const size_t rn = (size_t)R * n * sizeof(double);
+    B2nOutStage<3> O{{mean, cov, quant}, {rn, rn * n, rn * nq}};
+    B2N_TRY(O.bind(ctx));
+    J.mean = (double*)O.dev[0]; J.cov = (double*)O.dev[1]; J.quant = (double*)O.dev[2];
 
     B2N_TIME_BEGIN(ctx);
     transpose_kernel<<<dim3((unsigned)((N + 31) / 32), (unsigned)((R + 31) / 32)), dim3(32, 8), 0, ctx->stream>>>(
@@ -506,11 +472,12 @@ extern "C" int b2n_weighted_stats(b2n_ctx* ctx, const double* x, int64_t N, int3
 }
 
 namespace {
-// The common part of the realisation entries: x staged, shift from logwt_ref, outputs staged; `produce` enqueues the
-// producer that fills J.W / J.w2 / J.nw2 and the summaries and returns the record's logwt on the device.
+// The common part of the realisation entries: x staged, outputs staged, shift from logwt_ref; `produce` stages the
+// record, starts the timer and enqueues the producer that fills J.W / J.w2 / J.nw2 and the summaries, and returns the
+// record's logwt on the device.
 template <class Producer>
-int post_realisations(b2n_ctx* ctx, int64_t N, const double* x, int32_t n, int32_t R,
-                      const double* q, int32_t nq, double* const sum_user[4], double* mean, double* cov, double* quant,
+int post_realisations(b2n_ctx* ctx, int64_t N, const double* x, int32_t n, int32_t R, const double* q, int32_t nq,
+                      double* logz, double* logzerr, double* h, double* kld, double* mean, double* cov, double* quant,
                       Producer produce) {
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     PostJob J;
@@ -531,26 +498,19 @@ int post_realisations(b2n_ctx* ctx, int64_t N, const double* x, int32_t n, int32
             J.q = c + n;
         }
     }
-    void* d;
-    double* sum_dev[4];
-    DevBuf* const sum_buf[4] = {&ctx->out4, &ctx->out5, &ctx->out6, &ctx->out7};
-    for (int k = 0; k < 4; k++) {
-        B2N_TRY(b2n_out(ctx, *sum_buf[k], sum_user[k], (size_t)R * sizeof(double), &d));
-        sum_dev[k] = (double*)d;
-    }
-    PostOut O;
-    B2N_TRY(O.stage(ctx, mean, cov, quant, R, n, nq));
-    J.mean = O.dev[0]; J.cov = O.dev[1]; J.quant = O.dev[2];
+    const size_t rb = (size_t)R * sizeof(double), rn = rb * n;
+    B2nOutStage<7> O{{logz, logzerr, h, kld, mean, cov, quant}, {rb, rb, rb, rb, rn, rn * n, rn * nq}};
+    B2N_TRY(O.bind(ctx));
+    double* const sum[4] = {(double*)O.dev[0], (double*)O.dev[1], (double*)O.dev[2], (double*)O.dev[3]};
+    J.mean = (double*)O.dev[4]; J.cov = (double*)O.dev[5]; J.quant = (double*)O.dev[6];
 
-    B2N_TIME_BEGIN(ctx);
     const double* wref = nullptr;
-    B2N_TRY(produce(sum_dev, Wt, J, &wref));
+    B2N_TRY(produce(sum, Wt, &J.w2, &J.nw2, &wref));
     shift_kernel<<<(n + 31) / 32, 512, 0, ctx->stream>>>(wref, J.x, N, n, c);
     B2N_LAUNCH_CHECK(ctx);
     B2N_TRY(post_launch(ctx, J));
     B2N_TIME_END(ctx);
 
-    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], sum_dev[k], (size_t)R * sizeof(double)));
     B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);
 }
@@ -563,11 +523,10 @@ extern "C" int b2n_jitter_posterior(b2n_ctx* ctx, const double* logl, const int6
                                     double* quant) {
     if (!ctx || !logl || !samples_n || !logwt_ref) return B2N_ERR_ARG;
     B2N_TRY(post_check(N, n, R, x, nq, q, quant));
-    double* const sum_user[4] = {logz, logzerr, h, kld};
-    return post_realisations(ctx, N, x, n, R, q, nq, sum_user, mean, cov, quant,
-                             [&](double* const sum[4], double* W, PostJob& J, const double** wref) {
-                                 return b2n_jitter_weights(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R,
-                                                           seed, chain0, sum, W, (double**)&J.w2, &J.nw2, wref);
+    return post_realisations(ctx, N, x, n, R, q, nq, logz, logzerr, h, kld, mean, cov, quant,
+                             [&](double* const sum[4], double* W, const double** w2, int64_t* nw2, const double** wref) {
+                                 return b2n_jitter_produce(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R,
+                                                           seed, chain0, sum, nullptr, W, w2, nw2, wref);
                              });
 }
 
@@ -579,12 +538,10 @@ extern "C" int b2n_resample_posterior(b2n_ctx* ctx, const double* logl, const in
                                       double* cov, double* quant) {
     if (!ctx || !logl || !strand || !base || !piece_ptr || !logwt_ref || S < 1) return B2N_ERR_ARG;
     B2N_TRY(post_check(N, n, R, x, nq, q, quant));
-    double* const sum_user[4] = {logz, logzerr, h, kld};
-    return post_realisations(ctx, N, x, n, R, q, nq, sum_user, mean, cov, quant,
-                             [&](double* const sum[4], double* W, PostJob& J, const double** wref) {
-                                 J.nw2 = 1;
-                                 return b2n_resample_weights(ctx, logl, strand, N, S, base, piece_ptr, piece_strand,
-                                                             end, logwt_ref, logz_ref, R, seed, chain0, sum, W,
-                                                             (double**)&J.w2, wref);
+    return post_realisations(ctx, N, x, n, R, q, nq, logz, logzerr, h, kld, mean, cov, quant,
+                             [&](double* const sum[4], double* W, const double** w2, int64_t* nw2, const double** wref) {
+                                 return b2n_resample_produce(ctx, logl, strand, N, S, base, piece_ptr, piece_strand,
+                                                             end, logwt_ref, logz_ref, R, seed, chain0, sum, nullptr,
+                                                             W, w2, nw2, wref);
                              });
 }

@@ -12,7 +12,12 @@
 //                                          in the realisation (its logl is the previous copy's), ln X and logz
 //                                          before each sample; a thread then walks the m copies of its sample.
 // Nothing R x N is stored; a realisation never reads another's data, so it does not depend on R.
+//
+// Host side: b2n_resample_produce checks and stages a record and enqueues the two launches, for b2n_resample_runs
+// (below) and for b2n_resample_posterior (b2n_posterior.cu, with the weights); the entry points stage their outputs
+// through B2nOutStage (b2n_common.cuh).  The block scan and its operators are b2n_scan.cuh's.
 #include "b2n_device.cuh"
+#include "b2n_scan.cuh"
 
 #include <algorithm>
 #include <math.h>
@@ -42,62 +47,6 @@ struct RArgs {
                                  // -0.0 for a sample not drawn (resample_weights_kernel only)
     double* w2;                  // R: sum over the copies of exp(logwt - logz[-1])^2 (resample_weights_kernel only)
 };
-
-__device__ __forceinline__ double lae(double a, double b) {     // np.logaddexp
-    if (a == -INFINITY) return b;
-    if (b == -INFINITY) return a;
-    const double m = fmax(a, b);
-    return m + log1p(exp(-fabs(a - b)));
-}
-struct OpSum {
-    __device__ static double id() { return 0.0; }
-    __device__ double operator()(double a, double b) const { return a + b; }
-};
-struct OpLae {
-    __device__ static double id() { return -INFINITY; }
-    __device__ double operator()(double a, double b) const { return lae(a, b); }
-};
-struct OpMax {
-    __device__ static double id() { return -1.0; }
-    __device__ double operator()(double a, double b) const { return fmax(a, b); }
-};
-
-// In-place inclusive scan of x[0, n) (shared memory, n <= RS_TILE) with a fixed association: thread t owns a
-// contiguous run, then warp shuffles, then the warp totals.  Returns the total (identity for n == 0) to every thread.
-template <class Op>
-__device__ double block_scan(double* x, int n, double* wsum, Op op) {
-    const int t = threadIdx.x, lane = t & 31, w = t >> 5, nw = blockDim.x >> 5;
-    const int ipt = (n + blockDim.x - 1) / blockDim.x;
-    const int i0 = min(t * ipt, n), i1 = min(i0 + ipt, n);
-    double acc = Op::id();
-    for (int i = i0; i < i1; i++) { acc = op(acc, x[i]); x[i] = acc; }
-    double v = acc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const double u = __shfl_up_sync(B2N_FULL, v, o);
-        if (lane >= o) v = op(u, v);
-    }
-    if (lane == 31) wsum[w] = v;
-    __syncthreads();
-    if (w == 0) {
-        double s = lane < nw ? wsum[lane] : Op::id();
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const double u = __shfl_up_sync(B2N_FULL, s, o);
-            if (lane >= o) s = op(u, s);
-        }
-        if (lane < nw) wsum[lane] = s;
-    }
-    __syncthreads();
-    double ex = __shfl_up_sync(B2N_FULL, v, 1);
-    if (lane == 0) ex = Op::id();
-    if (w > 0) ex = op(wsum[w - 1], ex);
-    if (t > 0)
-        for (int i = i0; i < i1; i++) x[i] = op(ex, x[i]);
-    const double total = wsum[nw - 1];
-    __syncthreads();
-    return total;
-}
 
 __global__ void __launch_bounds__(RS_BLOCK) resample_mult_kernel(RArgs A) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
@@ -257,11 +206,13 @@ __device__ __forceinline__ void resample_scan(const RArgs& A) {
 __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) { resample_scan<false>(A); }
 __global__ void __launch_bounds__(RS_BLOCK) resample_weights_kernel(RArgs A) { resample_scan<true>(A); }
 
-// The inputs of b2n_resample_runs staged into A, its multiplicities in `mult` (device, R x S) or in scratch1 (NULL),
-// followed there by R doubles for the w^2 sums when w2 is set; the output pointers are left NULL.
-int resample_setup(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S, const uint8_t* base,
-                   const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end, const double* logwt_ref,
-                   double logz_ref, int32_t R, uint64_t seed, uint64_t chain0, int32_t* mult, bool w2, RArgs& A) {
+}  // namespace
+
+int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                         const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
+                         const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
+                         double* const sum[4], int32_t* mult, double* w, const double** w2, int64_t* nw2,
+                         const double** wref) {
     if (piece_ptr[0] != 0 || piece_ptr[N] < 0 || (piece_ptr[N] > 0 && !piece_strand)) return B2N_ERR_ARG;
     for (int64_t i = 0; i < N; i++)
         if (strand[i] < 0 || strand[i] >= S || piece_ptr[i + 1] < piece_ptr[i]) return B2N_ERR_ARG;
@@ -273,8 +224,8 @@ int resample_setup(b2n_ctx* ctx, const double* logl, const int32_t* strand, int6
     for (int s = 0; s < S; s++) if (!base[s]) ids.push_back(s);
     const int nadd = S - nbase;
     if (nbase == 0) return b2n_fail(ctx, B2N_ERR_ARG, "b2n_resample_runs: the record has no base strand");
-    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
 
+    RArgs A;
     memset(&A, 0, sizeof(A));
     const void* p;
     B2N_TRY(b2n_in(ctx, ctx->in0, logl, (size_t)N * sizeof(double), &p));
@@ -292,34 +243,33 @@ int resample_setup(b2n_ctx* ctx, const double* logl, const int32_t* strand, int6
     B2N_TRY(b2n_in_host(ctx, ctx->scratch3, ids.data(), ids.size() * sizeof(int32_t), &p));
     A.base_ids = (const int32_t*)p;
     A.N = N; A.S = S; A.nbase = nbase; A.nadd = nadd; A.zref = logz_ref; A.seed = seed; A.chain0 = chain0; A.R = R;
+    // the multiplicities in `mult` or in scratch1, followed there by the R w^2 sums when the weights are asked for
     const size_t msz = (size_t)R * S * sizeof(int32_t), mpad = (msz + 255) / 256 * 256;
     if (mult) {
         A.mult = mult;
-        if (w2) {
+        if (w) {
             B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)R * sizeof(double)));
             A.w2 = ctx->scratch1.as<double>();
         }
     } else {
-        B2N_CUDA(ctx, ctx->scratch1.ensure(w2 ? mpad + (size_t)R * sizeof(double) : msz));
+        B2N_CUDA(ctx, ctx->scratch1.ensure(w ? mpad + (size_t)R * sizeof(double) : msz));
         A.mult = ctx->scratch1.as<int32_t>();
-        if (w2) A.w2 = (double*)((char*)ctx->scratch1.p + mpad);
+        if (w) A.w2 = (double*)((char*)ctx->scratch1.p + mpad);
     }
-    return B2N_OK;
-}
+    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
+    A.w = w;
+    if (w) { *w2 = A.w2; *nw2 = 1; *wref = A.wref; }
 
-// The two launches on the stream (the multiplicities zeroed first); pass 2 with the weights when A.w is set.
-int resample_launch(b2n_ctx* ctx, const RArgs& A, int32_t R) {
-    B2N_CUDA(ctx, cudaMemsetAsync(A.mult, 0, (size_t)R * A.S * sizeof(int32_t), ctx->stream));
+    B2N_TIME_BEGIN(ctx);
+    B2N_CUDA(ctx, cudaMemsetAsync(A.mult, 0, msz, ctx->stream));
     const dim3 grid((unsigned)((std::max(A.nbase, A.nadd) + RS_BLOCK - 1) / RS_BLOCK), (unsigned)R);
     resample_mult_kernel<<<grid, RS_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
-    if (A.w) resample_weights_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
+    if (w) resample_weights_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
     else resample_scan_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     return B2N_OK;
 }
-
-}  // namespace
 
 extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
                                  const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand,
@@ -328,43 +278,14 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
                                  double* kld, int32_t* mult) {
     if (!ctx || !logl || !strand || !base || !piece_ptr || N < 1 || S < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
     if (!logwt_ref && kld) return B2N_ERR_ARG;
-    void* d;
-    const size_t msz = (size_t)R * S * sizeof(int32_t);
-    int32_t* dmult = nullptr;
-    if (mult) {
-        B2N_TRY(b2n_out(ctx, ctx->out4, mult, msz, &d));
-        dmult = (int32_t*)d;
-    }
-    RArgs A;
-    B2N_TRY(resample_setup(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R, seed,
-                           chain0, dmult, false, A));
-    double* const sum_user[4] = {logz, logzerr, h, kld};
-    double** const sum_dev[4] = {&A.out_logz, &A.out_logzerr, &A.out_h, &A.out_kld};
-    DevBuf* const sum_buf[4] = {&ctx->out0, &ctx->out1, &ctx->out2, &ctx->out3};
-    for (int k = 0; k < 4; k++) {
-        B2N_TRY(b2n_out(ctx, *sum_buf[k], sum_user[k], (size_t)R * sizeof(double), &d));
-        *sum_dev[k] = (double*)d;
-    }
-
-    B2N_TIME_BEGIN(ctx);
-    B2N_TRY(resample_launch(ctx, A, R));
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    const size_t rb = (size_t)R * sizeof(double);
+    B2nOutStage<5> O{{logz, logzerr, h, kld, mult}, {rb, rb, rb, rb, (size_t)R * S * sizeof(int32_t)}};
+    B2N_TRY(O.bind(ctx));
+    double* const d[4] = {(double*)O.dev[0], (double*)O.dev[1], (double*)O.dev[2], (double*)O.dev[3]};
+    B2N_TRY(b2n_resample_produce(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R,
+                                 seed, chain0, d, (int32_t*)O.dev[4], nullptr, nullptr, nullptr, nullptr));
     B2N_TIME_END(ctx);
-
-    B2N_TRY(b2n_out_done(ctx, mult, A.mult, msz));
-    for (int k = 0; k < 4; k++) B2N_TRY(b2n_out_done(ctx, sum_user[k], *sum_dev[k], (size_t)R * sizeof(double)));
+    B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);
-}
-
-int b2n_resample_weights(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
-                         const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
-                         const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
-                         double* const sum[4], double* w, double** w2, const double** wref) {
-    RArgs A;
-    B2N_TRY(resample_setup(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R, seed,
-                           chain0, nullptr, true, A));
-    A.out_logz = sum[0]; A.out_logzerr = sum[1]; A.out_h = sum[2]; A.out_kld = sum[3];
-    A.w = w;
-    *w2 = A.w2;
-    *wref = A.wref;
-    return resample_launch(ctx, A, R);
 }

@@ -555,6 +555,45 @@ def ns_destroy(ctx=None):
 
 
 # ---- run uncertainties (include/b200nest.h, b2n_jitter_runs) ----------------------------------------------
+def _logwt_ref(logwt_ref, N):
+    wref = f64(logwt_ref)
+    if len(wref) != N:
+        raise ValueError("logwt_ref and logl differ in length")
+    return wref
+
+
+def _jitter_record(logl, samples_n, logwt_ref, kl):
+    """(logl, samples_n, logwt_ref) of a jitter call as the C API takes them; logwt_ref is None when kl is False."""
+    logl = f64(logl)
+    n = np.ascontiguousarray(samples_n, dtype=np.int64)
+    if len(n) != len(logl):
+        raise ValueError("logl and samples_n differ in length")
+    return logl, n, _logwt_ref(logwt_ref, len(logl)) if kl else None
+
+
+def _strand_record(N, strand, base, piece_ptr, piece_strand, end):
+    """(strand, base, piece_ptr, piece_strand, end) of a resample call over N samples as the C API takes them."""
+    strand = np.ascontiguousarray(strand, dtype=np.int32)
+    base = np.ascontiguousarray(base, dtype=np.uint8)
+    pp = np.ascontiguousarray(piece_ptr, dtype=np.int64)
+    ps = np.ascontiguousarray(piece_strand, dtype=np.int32)
+    if len(strand) != N or len(pp) != N + 1:
+        raise ValueError("logl, strand and piece_ptr differ in length")
+    if end is not None:
+        end = np.ascontiguousarray(end, dtype=np.uint8)
+        if len(end) != N:
+            raise ValueError("logl and end differ in length")
+    return strand, base, pp, ps, end
+
+
+def _summaries(R, kl):
+    """The per-realisation outputs logz, logzerr, h and, with kl, kld (R each)."""
+    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
+    if kl:
+        o['kld'] = np.empty(R)
+    return o
+
+
 def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, arrays=False,
                 ctx=None):
     """R prior-volume realisations of one record (jitter_run / kld_error, utils.py:1317-1408, 1932-1997); realisation
@@ -562,18 +601,10 @@ def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None
     last elements of the realisations' arrays) and, with arrays=True, logvol_arr, logwt_arr, logz_arr[, kld_arr]
     (R x N).  kld needs the input run's weights: logwt_ref (N) and logz_ref (its logz[-1])."""
     ctx = _ctx(ctx)
-    logl = f64(logl)
-    n = np.ascontiguousarray(samples_n, dtype=np.int64)
-    N, R = len(logl), int(R)
-    if len(n) != N:
-        raise ValueError("logl and samples_n differ in length")
     kl = logwt_ref is not None
-    wref = f64(logwt_ref) if kl else None
-    if kl and len(wref) != N:
-        raise ValueError("logwt_ref and logl differ in length")
-    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
-    if kl:
-        o['kld'] = np.empty(R)
+    logl, n, wref = _jitter_record(logl, samples_n, logwt_ref, kl)
+    N, R = len(logl), int(R)
+    o = _summaries(R, kl)
     if arrays:
         for k in ('logvol', 'logwt', 'logz') + (('kld',) if kl else ()):
             o[k + '_arr'] = np.empty((R, N))
@@ -595,24 +626,11 @@ def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, cha
     ctx = _ctx(ctx)
     logl = f64(logl)
     N = len(logl)
-    strand = np.ascontiguousarray(strand, dtype=np.int32)
-    base = np.ascontiguousarray(base, dtype=np.uint8)
-    pp = np.ascontiguousarray(piece_ptr, dtype=np.int64)
-    ps = np.ascontiguousarray(piece_strand, dtype=np.int32)
-    if len(strand) != N or len(pp) != N + 1:
-        raise ValueError("logl, strand and piece_ptr differ in length")
-    if end is not None:
-        end = np.ascontiguousarray(end, dtype=np.uint8)
-        if len(end) != N:
-            raise ValueError("logl and end differ in length")
+    strand, base, pp, ps, end = _strand_record(N, strand, base, piece_ptr, piece_strand, end)
     S, R = len(base), int(R)
     kl = logwt_ref is not None
-    wref = f64(logwt_ref) if kl else None
-    if kl and len(wref) != N:
-        raise ValueError("logwt_ref and logl differ in length")
-    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
-    if kl:
-        o['kld'] = np.empty(R)
+    wref = _logwt_ref(logwt_ref, N) if kl else None
+    o = _summaries(R, kl)
     m = np.empty((R, S), dtype=np.int32) if multiplicities else None
     ctx.check(ctx.lib.b2n_resample_runs(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps), ptr(end),
                                         ptr(wref), float(logz_ref) if kl else 0.0, R, int(seed), int(chain0),
@@ -673,17 +691,11 @@ def jitter_posterior(logl, samples_n, x, R, seed, chain0=0, approx=False, logwt_
     """jitter_runs plus, per realisation, the weighted mean (R x n), covariance (R x n x n) and, with q, quantiles
     (R x n x nq) of the sample positions x (N x n).  logwt_ref / logz_ref (the record's own) are required."""
     ctx = _ctx(ctx)
-    logl = f64(logl)
-    n_ = np.ascontiguousarray(samples_n, dtype=np.int64)
+    logl, n_, wref = _jitter_record(logl, samples_n, logwt_ref, True)
     N, R = len(logl), int(R)
-    if len(n_) != N:
-        raise ValueError("logl and samples_n differ in length")
-    wref = f64(logwt_ref)
-    if len(wref) != N:
-        raise ValueError("logwt_ref and logl differ in length")
     x = _post_x(x, N)
     q = _post_q(q)
-    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R), kld=np.empty(R))
+    o = _summaries(R, True)
     o.update(_post_outputs(R, x.shape[1], q, True))
     ctx.check(ctx.lib.b2n_jitter_posterior(ctx.h, ptr(logl), ptr(n_), N, ptr(wref), float(logz_ref),
                                            int(bool(approx)), R, int(seed), int(chain0), ptr(x), x.shape[1], ptr(q),
@@ -699,23 +711,12 @@ def resample_posterior(logl, strand, base, piece_ptr, piece_strand, end, x, R, s
     ctx = _ctx(ctx)
     logl = f64(logl)
     N = len(logl)
-    strand = np.ascontiguousarray(strand, dtype=np.int32)
-    base = np.ascontiguousarray(base, dtype=np.uint8)
-    pp = np.ascontiguousarray(piece_ptr, dtype=np.int64)
-    ps = np.ascontiguousarray(piece_strand, dtype=np.int32)
-    if len(strand) != N or len(pp) != N + 1:
-        raise ValueError("logl, strand and piece_ptr differ in length")
-    if end is not None:
-        end = np.ascontiguousarray(end, dtype=np.uint8)
-        if len(end) != N:
-            raise ValueError("logl and end differ in length")
+    strand, base, pp, ps, end = _strand_record(N, strand, base, piece_ptr, piece_strand, end)
     S, R = len(base), int(R)
-    wref = f64(logwt_ref)
-    if len(wref) != N:
-        raise ValueError("logwt_ref and logl differ in length")
+    wref = _logwt_ref(logwt_ref, N)
     x = _post_x(x, N)
     q = _post_q(q)
-    o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R), kld=np.empty(R))
+    o = _summaries(R, True)
     o.update(_post_outputs(R, x.shape[1], q, True))
     ctx.check(ctx.lib.b2n_resample_posterior(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps),
                                              ptr(end), ptr(wref), float(logz_ref), R, int(seed), int(chain0), ptr(x),

@@ -47,13 +47,17 @@ def samples_n_of(res):
     raise ValueError("Final number of samples differs from number of iterations and number of live points.")
 
 
+def _logz_end(res):
+    """The record's own logz[-1] (the reference weights' normalisation)."""
+    return float(np.asarray(res['logz'])[-1])
+
+
 def jitter_realisations(res, n_mc, seed, chain0=0, approx=False, arrays=False, ctx=None):
     """n_mc realisations of `res` in one call.  Returns dict(logz, logzerr, h, kld): the last element of each
     realisation's logz / logzerr / information / cumulative KL divergence (n_mc values each); with arrays=True also
     logvol_arr, logwt_arr, logz_arr, kld_arr (n_mc x nsamps).  Realisation r uses the stream (seed, chain0 + r)."""
-    logz = np.asarray(res['logz'])
     return ops.jitter_runs(res['logl'], samples_n_of(res), int(n_mc), int(seed), chain0=int(chain0),
-                           approx=approx, logwt_ref=res['logwt'], logz_ref=float(logz[-1]), arrays=arrays, ctx=ctx)
+                           approx=approx, logwt_ref=res['logwt'], logz_ref=_logz_end(res), arrays=arrays, ctx=ctx)
 
 
 def _realisation(res, seed, chain, approx, ctx):
@@ -165,19 +169,24 @@ def _piece_csr(logl, plan):
     return ptr_, pstr[np.argsort(start, kind='stable')]
 
 
+def _strand_inputs(res):
+    """(plan, record): the strand plan of `res` and the record as b2n_resample_runs takes it, (logl, strand, base,
+    piece_ptr, piece_strand, end).  The record must hold a strand started from the prior."""
+    plan = strand_plan(res)
+    if not plan['base'].any():
+        raise ValueError("The provided `Results` does not include any points initially sampled from the prior!")
+    logl = np.asarray(res['logl'], dtype=float)
+    return plan, (logl, plan['strand'], plan['base']) + _piece_csr(logl, plan) + (plan['end'],)
+
+
 def resample_realisations(res, n_mc, seed, chain0=0, multiplicities=False, ctx=None):
     """n_mc resample_run realisations of `res` in one call.  Returns dict(logz, logzerr, h, kld): the last element of
     each realisation's logz / logzerr / information / cumulative KL divergence (n_mc values each); with
     multiplicities=True also mult (n_mc x nstrands): the times each strand (in the order of np.unique(samples_id)) is
     drawn.  Realisation r uses the stream (seed, chain0 + r)."""
-    plan = strand_plan(res)
-    if not plan['base'].any():
-        raise ValueError("The provided `Results` does not include any points initially sampled from the prior!")
-    logl = np.asarray(res['logl'], dtype=float)
-    pptr, pstr = _piece_csr(logl, plan)
-    return ops.resample_runs(logl, plan['strand'], plan['base'], pptr, pstr, plan['end'], int(n_mc), int(seed),
-                             chain0=int(chain0), logwt_ref=res['logwt'], logz_ref=float(np.asarray(res['logz'])[-1]),
-                             multiplicities=multiplicities, ctx=ctx)
+    rec = _strand_inputs(res)[1]
+    return ops.resample_runs(*rec, int(n_mc), int(seed), chain0=int(chain0), logwt_ref=res['logwt'],
+                             logz_ref=_logz_end(res), multiplicities=multiplicities, ctx=ctx)
 
 
 def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
@@ -186,10 +195,10 @@ def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
     batch) among themselves -- with the live counts of the strand rule and the integrals of those.  The draw is the
     stream (seed, chain) (b2n_resample_runs computes it and the summaries; the arrays are built here).  With
     return_idx, also the index in `res` of every sample of the new run."""
-    plan = strand_plan(res)
-    o = resample_realisations(res, 1, _seed(seed), chain, multiplicities=True, ctx=ctx)
-    m = o['mult'][0]
-    logl = np.asarray(res['logl'], dtype=float)
+    plan, rec = _strand_inputs(res)
+    m = ops.resample_runs(*rec, 1, _seed(seed), chain0=int(chain), logwt_ref=res['logwt'], logz_ref=_logz_end(res),
+                          multiplicities=True, ctx=ctx)['mult'][0]
+    logl = rec[0]
     N = len(logl)
     start, pstr = _pieces(logl, plan)
     ms = m[plan['strand']]
@@ -294,17 +303,12 @@ def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=Fal
     if x.ndim != 2 or len(x) != len(logl) or x.shape[1] < 1:
         raise ValueError("posterior_realisations needs the sample positions of every point (res['samples']); "
                          "a run made with keep_samples=False has none")
-    logz_ref = float(np.asarray(res['logz'])[-1])
+    logz_ref = _logz_end(res)
     if error == 'jitter':
         return ops.jitter_posterior(logl, samples_n_of(res), x, int(n_mc), int(seed), chain0=int(chain0),
                                     approx=approx, logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx)
-    plan = strand_plan(res)
-    if not plan['base'].any():
-        raise ValueError("The provided `Results` does not include any points initially sampled from the prior!")
-    pptr, pstr = _piece_csr(logl, plan)
-    return ops.resample_posterior(logl, plan['strand'], plan['base'], pptr, pstr, plan['end'], x, int(n_mc),
-                                  int(seed), chain0=int(chain0), logwt_ref=res['logwt'], logz_ref=logz_ref, q=q,
-                                  ctx=ctx)
+    return ops.resample_posterior(*_strand_inputs(res)[1], x, int(n_mc), int(seed), chain0=int(chain0),
+                                  logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx)
 
 
 # ---------------------------------------------------------------------------------------------- merging runs
