@@ -145,6 +145,8 @@ SYMBOLS = {
     'b2n_resample_posterior': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _I, _P, _I,
                                          _P, _P, _P, _P, _P, _P, _P]),
     'b2n_merge_runs': (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'b2n_compute_integrals': (C.c_int, [_P, _P, _P, _P, _L, _P, _P, _P, _P, _P]),
+    'b2n_set_reweight': (C.c_int, [_P, _P, _L]),
 }
 
 _lib = None
@@ -247,6 +249,10 @@ class Context:
     def set_start_rows(self, idx_ptr, nrows):
         """the next rwalk call takes its start points as rows idx[q] of its u0 (= the whole live set)"""
         self.check(self.lib.b2n_set_start_rows(self.h, idx_ptr, int(nrows)))
+
+    def set_reweight(self, logrwt_ptr, n):
+        """the next jitter / resample realisation call adds logrwt (n) to every logwt"""
+        self.check(self.lib.b2n_set_reweight(self.h, logrwt_ptr, int(n)))
 
     def synchronize(self):
         self.check(self.lib.b2n_synchronize(self.h))

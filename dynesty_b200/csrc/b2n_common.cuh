@@ -130,6 +130,8 @@ struct b2n_ctx {
     void* friends = nullptr;    // resident RadFriends / SupFriends bound (b2n_friends.cu)
     const int32_t* start_idx = nullptr;   // b2n_set_start_rows: the NEXT rwalk call reads its start points as rows of u0
     int64_t start_nrows = 0;
+    const double* reweight = nullptr;    // b2n_set_reweight: the NEXT realisation call adds it to every logwt
+    int64_t reweight_n = 0;
     int min_cpc = 1;            // b2n_set_chain_pack: at least this many chains per CTA (see include/b200nest.h)
     int bound_fast_skip = 0;    // b2n_multi_decompose: updates left to skip the Cholesky candidate path
     // speculative eigen fit of the root node, concurrent with the candidate tree (b2n_bounding.cu: b2n_spec_root_*)
@@ -168,26 +170,29 @@ void b2n_ns_release(b2n_ctx* ctx);
 void b2n_friends_release(b2n_ctx* ctx);
 int b2n_bound_set_dev(b2n_ctx* ctx, int K, int nc, const double* dctrs, const double* dams, const double* daxes,
                       const double* h_logvols);
-// compute_integrals of one record with given ln t per sample, on the passes of b2n_jitter_runs (b2n_jitter.cu).
-// Device pointers; uses ctx->scratch0 / scratch1; does not synchronise.
-int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
-                      double* logwt, double* logz, double* logzvar, double* h);
+// compute_integrals of one record with given ln t per sample, and optionally a log-reweight lrw (N) added to every
+// logwt, on the passes of b2n_jitter_runs (b2n_jitter.cu).  Device pointers; uses ctx->scratch0 / scratch1; does not
+// synchronise.
+int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, const double* lrw, int64_t N, double* last3,
+                      double* logvol, double* logwt, double* logz, double* logzvar, double* h);
 // The realisations of b2n_jitter_runs (b2n_jitter.cu): the record staged, the call's timer started (B2N_TIME_BEGIN),
-// the passes enqueued; no synchronisation.  sum[4]: logz, logzerr, h, kld (R each); full: NULL or logvol, logwt, logz,
+// the passes enqueued; no synchronisation.  logrwt: NULL or the log-reweight (N) added to every logwt, staged in
+// ctx->work1.  sum[4]: logz, logzerr, h, kld (R each); full: NULL or logvol, logwt, logz,
 // kld (R x N each); device pointers, each may be NULL.  With w (device, N x R), pass 2 also writes the weights
 // exp(logwt - logz[-1]) and the per-segment sums of their squares, *w2 (R x *nw2, in ctx->scratch1), and *wref is the
 // record's logwt on the device.  Uses ctx->in0..in3, scratch0 and scratch1.
 int b2n_jitter_produce(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
-                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, double* const sum[4],
-                       double* const full[4], double* w, const double** w2, int64_t* nw2, const double** wref);
+                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, const double* logrwt,
+                       double* const sum[4], double* const full[4], double* w, const double** w2, int64_t* nw2,
+                       const double** wref);
 // The same for b2n_resample_runs (b2n_resample.cu): mult, the multiplicities (device, R x S), may be NULL (then they
 // live in ctx->scratch1); with w, the weights are -0.0 for a sample not drawn and *w2 holds R sums (*nw2 = 1).  Uses
 // ctx->in0..in3 and scratch0..scratch3.
 int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
                          const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
                          const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
-                         double* const sum[4], int32_t* mult, double* w, const double** w2, int64_t* nw2,
-                         const double** wref);
+                         const double* logrwt, double* const sum[4], int32_t* mult, double* w, const double** w2,
+                         int64_t* nw2, const double** wref);
 
 void b2n_peer_release(b2n_ctx* ctx);
 
@@ -337,6 +342,31 @@ struct B2nOutStage {
         return B2N_OK;
     }
 };
+// The log-reweight of b2n_set_reweight / b2n_compute_integrals: in host-pointer mode NaN and +inf are refused (device
+// arrays are the caller's to check).
+static inline int b2n_reweight_check(b2n_ctx* ctx, const double* lrw, int64_t N) {
+    if (!lrw || ctx->ptr_mode == B2N_PTR_DEVICE) return B2N_OK;
+    for (int64_t i = 0; i < N; i++)
+        if (!(lrw[i] < INFINITY)) return b2n_fail(ctx, B2N_ERR_ARG, "the log-reweight holds NaN or +inf");
+    return B2N_OK;
+}
+// A realisation entry point takes the pending b2n_set_reweight, clearing it however the call ends: *lrw = it or NULL.
+// It must have been set for the same N.
+static inline int b2n_take_reweight(b2n_ctx* ctx, int64_t N, const double** lrw) {
+    *lrw = ctx->reweight;
+    const int64_t n = ctx->reweight_n;
+    ctx->reweight = nullptr; ctx->reweight_n = 0;
+    if (*lrw && n != N) return b2n_fail(ctx, B2N_ERR_ARG, "b2n_set_reweight was given another number of samples");
+    return B2N_OK;
+}
+// The run-statistics entry points that do not read a pending b2n_set_reweight refuse and clear it.
+static inline int b2n_refuse_reweight(b2n_ctx* ctx, const char* who) {
+    if (!ctx->reweight) return B2N_OK;
+    ctx->reweight = nullptr; ctx->reweight_n = 0;
+    snprintf(ctx->err, sizeof(ctx->err), "%s does not read a log-reweight (b2n_set_reweight is read by the jitter / "
+             "resample realisation entry points only)", who);
+    return B2N_ERR_UNSUPPORTED;
+}
 static inline int b2n_finish(b2n_ctx* ctx) {
     if (ctx->ptr_mode == B2N_PTR_HOST) B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2N_OK;

@@ -184,6 +184,15 @@ int b2n_set_start_rows(b2n_ctx* ctx, const int32_t* idx, int64_t nrows) {
     return B2N_OK;
 }
 
+int b2n_set_reweight(b2n_ctx* ctx, const double* logrwt, int64_t N) {
+    if (!ctx || (logrwt && N < 1)) return B2N_ERR_ARG;
+    ctx->reweight = nullptr; ctx->reweight_n = 0;
+    B2N_TRY(b2n_reweight_check(ctx, logrwt, N));
+    ctx->reweight = logrwt;
+    ctx->reweight_n = logrwt ? N : 0;
+    return B2N_OK;
+}
+
 int b2n_set_chain_pack(b2n_ctx* ctx, int32_t chains_per_cta) {
     if (!ctx || chains_per_cta < 1) return B2N_ERR_ARG;
     ctx->min_cpc = chains_per_cta;

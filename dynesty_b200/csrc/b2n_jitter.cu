@@ -22,7 +22,9 @@
 //                            A and C to the full h and logzvar arrays (b2n_integrate_lnt only)
 //
 // b2n_integrate_lnt (below, for b2n_merge.cu) runs the same passes in a deterministic mode: one realisation whose ln t
-// per sample is read from an array (segment_lnt<true>), over a plan of tick-0 segments only.
+// per sample is read from an array (segment_lnt<true>), over a plan of tick-0 segments only; b2n_compute_integrals
+// (below) runs that mode on ln t = diff(logvol).  With a log-reweight (A.lrw, b2n_set_reweight) the passes run their
+// _rw instantiations, which add it to every logwt.
 //
 // Host side: b2n_jitter_produce stages a record and enqueues the passes, for b2n_jitter_runs (below) and for
 // b2n_jitter_posterior (b2n_posterior.cu, with the weights of pass 2); the entry points stage their outputs through
@@ -64,6 +66,7 @@ struct JArgs {
     double* f_h; double* f_logzvar;                      // N, may be NULL (b2n_integrate_lnt only)
     double* f_w;             // N x R (sample-major): w = exp(logwt - logz[-1]) (jitter_weights_kernel only)
     double* s_w2;            // R x nseg: segment sums of w^2 (jitter_weights_kernel only)
+    const double* lrw;       // N: log-reweight added to every logwt (the _rw kernels only), else NULL
 };
 
 // ln t of the segment's samples into lt[0, len)
@@ -104,8 +107,11 @@ __device__ void segment_lnt(const JArgs& A, const JSeg& s, int r, double* lt, do
 
 // GIVEN: ln t read from A.lnt (b2n_integrate_lnt); the full h / logzvar arrays are written only in that mode, so the
 // instantiations of b2n_jitter_runs compile to the code they had before it existed.  WOUT (pass 2 only): also the
-// weights f_w and the segment sums of their squares s_w2 (b2n_jitter_posterior), likewise only in that mode.
-template <int PASS, bool GIVEN, bool WOUT>
+// weights f_w and the segment sums of their squares s_w2 (b2n_jitter_posterior), likewise only in that mode.  RW: lrw[j]
+// is added to every logwt (pass 1's local weights, pass 2's cap), so logz, the KL terms and the weights are the
+// reweighted ones while the h increments keep the unreweighted L and ldv2 (compute_integrals(reweight=)); a KL term of
+// zero weight is 0.  Without RW the code is the one it was before the reweight existed.
+template <int PASS, bool GIVEN, bool WOUT, bool RW = false>
 __device__ __forceinline__ void jitter_pass(const JArgs& A) {
     __shared__ double lt[JT_TILE], pv[JT_TILE], cap[JT_TILE + 1], buf[JT_CHUNK], wsum[32];
     const int64_t sg = blockIdx.x;
@@ -123,6 +129,7 @@ __device__ __forceinline__ void jitter_pass(const JArgs& A) {
             const int64_t j = s.a + i;
             const double lprev = j > 0 ? A.logl[j - 1] : -1e300;
             buf[i] = (i > 0 ? pv[i - 1] : 0.0) + lae(A.logl[j], lprev) + log1p(-exp(lt[i])) + ln_half;
+            if (RW) buf[i] += A.lrw[j];
         }
         __syncthreads();
         const double E = block_scan(buf, L, wsum, OpLae());
@@ -137,6 +144,10 @@ __device__ __forceinline__ void jitter_pass(const JArgs& A) {
         const double lprev = j > 0 ? A.logl[j - 1] : -1e300;
         cap[i] = lae(A.logl[j], lprev) + V + (i > 0 ? pv[i - 1] : 0.0) + log1p(-exp(lt[i])) + ln_half;
         buf[i] = cap[i];
+    }
+    if (RW) {
+        __syncthreads();
+        for (int i = threadIdx.x; i < L; i += blockDim.x) buf[i] = cap[i] += A.lrw[s.a + i];
     }
     __syncthreads();
     block_scan(buf, L, wsum, OpLae());
@@ -161,7 +172,7 @@ __device__ __forceinline__ void jitter_pass(const JArgs& A) {
         c_r[u] = dh * -lt[i];
         if (!GIVEN && A.wref) {             // (no KL divergence against given ln t)
             const double lp1 = cap[i] - zmax;
-            k_r[u] = exp(lp1) * (lp1 - (A.wref[j] - A.zref));
+            if (!RW || lp1 != -INFINITY) k_r[u] = exp(lp1) * (lp1 - (A.wref[j] - A.zref));
         }
         if (WOUT) {
             const double w = exp(cap[i] - zmax);
@@ -208,6 +219,11 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_pass_kernel(JArgs A) { jitter
 
 // Pass 2 of b2n_jitter_posterior: jitter_pass_kernel<2, false> plus the weights.
 __global__ void __launch_bounds__(JT_BLOCK) jitter_weights_kernel(JArgs A) { jitter_pass<2, false, true>(A); }
+
+// The same two with the log-reweight A.lrw (b2n_set_reweight, b2n_compute_integrals).
+template <int PASS, bool GIVEN>
+__global__ void __launch_bounds__(JT_BLOCK) jitter_pass_rw_kernel(JArgs A) { jitter_pass<PASS, GIVEN, false, true>(A); }
+__global__ void __launch_bounds__(JT_BLOCK) jitter_weights_rw_kernel(JArgs A) { jitter_pass<2, false, true, true>(A); }
 
 // One realisation per block: running scans over its segments in chunks of JT_TILE.
 // PASS 1: logvol (sV) and logz (sZ) before every segment, zend = logz[-1].
@@ -296,14 +312,15 @@ __global__ void __launch_bounds__(JT_BLOCK) jitter_offsets_kernel(JArgs A) {
 // The passes on the stream for a prepared JArgs (seg, nseg, N, R and the scratch pointers set).
 int jitter_launch(b2n_ctx* ctx, const JArgs& A, bool given) {
     const dim3 grid((unsigned)A.nseg, (unsigned)A.R);
-    if (given) jitter_pass_kernel<1, true><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-    else jitter_pass_kernel<1, false><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    const bool rw = A.lrw != nullptr;
+    if (given) (rw ? jitter_pass_rw_kernel<1, true> : jitter_pass_kernel<1, true>)<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else (rw ? jitter_pass_rw_kernel<1, false> : jitter_pass_kernel<1, false>)<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     jitter_scan_kernel<1><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
-    if (given) jitter_pass_kernel<2, true><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-    else if (A.f_w) jitter_weights_kernel<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
-    else jitter_pass_kernel<2, false><<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    if (given) (rw ? jitter_pass_rw_kernel<2, true> : jitter_pass_kernel<2, true>)<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else if (A.f_w) (rw ? jitter_weights_rw_kernel : jitter_weights_kernel)<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
+    else (rw ? jitter_pass_rw_kernel<2, false> : jitter_pass_kernel<2, false>)<<<grid, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     jitter_scan_kernel<2><<<A.R, JT_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
@@ -369,8 +386,9 @@ int jitter_plan(const int64_t* n, int64_t N, int approx, std::vector<JSeg>& seg,
 }  // namespace
 
 int b2n_jitter_produce(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
-                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, double* const sum[4],
-                       double* const full[4], double* w, const double** w2, int64_t* nw2, const double** wref) {
+                       double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, const double* logrwt,
+                       double* const sum[4], double* const full[4], double* w, const double** w2, int64_t* nw2,
+                       const double** wref) {
     std::vector<JSeg> seg;
     std::vector<int32_t> aux;
     B2N_TRY(jitter_plan(samples_n, N, approx, seg, aux));
@@ -386,6 +404,8 @@ int b2n_jitter_produce(b2n_ctx* ctx, const double* logl, const int64_t* samples_
     A.logl = (const double*)p;
     B2N_TRY(b2n_in(ctx, ctx->in1, logwt_ref, logwt_ref ? (size_t)N * sizeof(double) : 0, &p));
     A.wref = (const double*)p;
+    B2N_TRY(b2n_in(ctx, ctx->work1, logrwt, logrwt ? (size_t)N * sizeof(double) : 0, &p));
+    A.lrw = (const double*)p;
     B2N_TRY(b2n_in_host(ctx, ctx->in2, nl.data(), (size_t)N * sizeof(int32_t), &p));
     A.nlive = (const int32_t*)p;
     B2N_TRY(b2n_in_host(ctx, ctx->in3, aux.data(), (size_t)N * sizeof(int32_t), &p));
@@ -407,7 +427,10 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
                                const double* logwt_ref, double logz_ref, int32_t approx, int32_t R, uint64_t seed,
                                uint64_t chain0, double* logz, double* logzerr, double* h, double* kld,
                                double* logvol_full, double* logwt_full, double* logz_full, double* kld_full) {
-    if (!ctx || !logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    const double* logrwt;
+    B2N_TRY(b2n_take_reweight(ctx, N, &logrwt));
+    if (!logl || !samples_n || N < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
     if (!logwt_ref && (kld || kld_full)) return B2N_ERR_ARG;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t rb = (size_t)R * sizeof(double), fb = rb * N;
@@ -416,19 +439,19 @@ extern "C" int b2n_jitter_runs(b2n_ctx* ctx, const double* logl, const int64_t* 
     B2N_TRY(O.bind(ctx));
     double* d[8];
     for (int k = 0; k < 8; k++) d[k] = (double*)O.dev[k];
-    B2N_TRY(b2n_jitter_produce(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, d, d + 4, nullptr,
-                               nullptr, nullptr, nullptr));
+    B2N_TRY(b2n_jitter_produce(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R, seed, chain0, logrwt, d, d + 4,
+                               nullptr, nullptr, nullptr, nullptr));
     B2N_TIME_END(ctx);
     B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);
 }
 
 // compute_integrals (utils.py:1411-1467) of one record whose ln t per sample is given: logvol = cumsum(lnt), then the
-// quadrature of the passes above.  Every pointer is a device pointer; the outputs may be NULL.  last3 (3 doubles):
-// logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1].  Enqueues on the context's stream and does not synchronise; uses
-// ctx->scratch0 and ctx->scratch1.
-int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64_t N, double* last3, double* logvol,
-                      double* logwt, double* logz, double* logzvar, double* h) {
+// quadrature of the passes above, with the log-reweight lrw (N, or NULL) added to every logwt.  Every pointer is a
+// device pointer; the outputs may be NULL.  last3 (3 doubles): logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|), h[-1].
+// Enqueues on the context's stream and does not synchronise; uses ctx->scratch0 and ctx->scratch1.
+int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, const double* lrw, int64_t N, double* last3,
+                      double* logvol, double* logwt, double* logz, double* logzvar, double* h) {
     std::vector<JSeg> seg;
     for (int64_t a = 0; a < N; a += JT_TILE) seg.push_back(JSeg{a, (int32_t)std::min<int64_t>(JT_TILE, N - a), 0, 0});
     if ((int64_t)seg.size() > INT32_MAX) return B2N_ERR_ARG;
@@ -437,10 +460,45 @@ int b2n_integrate_lnt(b2n_ctx* ctx, const double* logl, const double* lnt, int64
     const void* p;
     B2N_TRY(b2n_in_host(ctx, ctx->scratch0, seg.data(), seg.size() * sizeof(JSeg), &p));
     A.seg = (const JSeg*)p;
-    A.logl = logl; A.lnt = lnt;
+    A.logl = logl; A.lnt = lnt; A.lrw = lrw;
     A.N = N; A.nseg = (int64_t)seg.size(); A.R = 1;
     B2N_TRY(jitter_scratch(ctx, A));
     if (last3) { A.out_logz = last3; A.out_logzerr = last3 + 1; A.out_h = last3 + 2; }
     A.f_logvol = logvol; A.f_logwt = logwt; A.f_logz = logz; A.f_logzvar = logzvar; A.f_h = h;
     return jitter_launch(ctx, A, true);
+}
+
+namespace {
+// ln t = diff(logvol, prepend=0): the volumes of compute_integrals as the deterministic passes read them
+__global__ void __launch_bounds__(JT_BLOCK) logvol_diff_kernel(const double* logvol, int64_t N, double* lnt) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N) lnt[i] = i > 0 ? logvol[i] - logvol[i - 1] : logvol[0];
+}
+}  // namespace
+
+extern "C" int b2n_compute_integrals(b2n_ctx* ctx, const double* logl, const double* logvol, const double* logrwt,
+                                     int64_t N, double* last3, double* logwt, double* logz, double* logzvar,
+                                     double* h) {
+    if (!ctx) return B2N_ERR_ARG;
+    B2N_TRY(b2n_refuse_reweight(ctx, "b2n_compute_integrals"));
+    if (!logl || !logvol || N < 1 || (N + JT_BLOCK - 1) / JT_BLOCK > INT32_MAX) return B2N_ERR_ARG;
+    B2N_TRY(b2n_reweight_check(ctx, logrwt, N));
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    const size_t nb = (size_t)N * sizeof(double);
+    B2nOutStage<5> O{{last3, logwt, logz, logzvar, h}, {3 * sizeof(double), nb, nb, nb, nb}};
+    B2N_TRY(O.bind(ctx));
+    const void *dl, *dv, *dr;
+    B2N_TRY(b2n_in(ctx, ctx->in0, logl, nb, &dl));
+    B2N_TRY(b2n_in(ctx, ctx->in1, logvol, nb, &dv));
+    B2N_TRY(b2n_in(ctx, ctx->work1, logrwt, logrwt ? nb : 0, &dr));
+    B2N_CUDA(ctx, ctx->in2.ensure(nb));
+    double* lnt = ctx->in2.as<double>();
+    B2N_TIME_BEGIN(ctx);
+    logvol_diff_kernel<<<(unsigned)((N + JT_BLOCK - 1) / JT_BLOCK), JT_BLOCK, 0, ctx->stream>>>((const double*)dv, N, lnt);
+    B2N_LAUNCH_CHECK(ctx);
+    B2N_TRY(b2n_integrate_lnt(ctx, (const double*)dl, lnt, (const double*)dr, N, (double*)O.dev[0], nullptr,
+                              (double*)O.dev[1], (double*)O.dev[2], (double*)O.dev[3], (double*)O.dev[4]));
+    B2N_TIME_END(ctx);
+    B2N_TRY(O.done(ctx));
+    return b2n_finish(ctx);
 }

@@ -121,7 +121,9 @@ inline unsigned blocks(int64_t n) { return (unsigned)((n + MG_BLOCK - 1) / MG_BL
 extern "C" int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, const int64_t* run_ptr,
                               int32_t R, int32_t nbase, const double* lowedge, int64_t* perm, int64_t* samples_n_out,
                               double* last3, double* logvol, double* logwt, double* logz, double* logzvar, double* h) {
-    if (!ctx || !logl || !samples_n || !run_ptr || R < 1 || nbase < 1 || nbase > R) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    B2N_TRY(b2n_refuse_reweight(ctx, "b2n_merge_runs"));
+    if (!logl || !samples_n || !run_ptr || R < 1 || nbase < 1 || nbase > R) return B2N_ERR_ARG;
     if (run_ptr[0] != 0) return B2N_ERR_ARG;
     for (int32_t r = 0; r < R; r++) {
         if (run_ptr[r + 1] <= run_ptr[r]) return B2N_ERR_ARG;            // every run holds a sample
@@ -202,7 +204,7 @@ extern "C" int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* s
     const MBuf m = b[cur];
     merge_lnt_kernel<<<blocks(N), MG_BLOCK, 0, ctx->stream>>>(m.logl, m.n, N, d_lnt);
     B2N_LAUNCH_CHECK(ctx);
-    B2N_TRY(b2n_integrate_lnt(ctx, m.logl, d_lnt, N, fd[0], fd[1], fd[2], fd[3], fd[4], fd[5]));
+    B2N_TRY(b2n_integrate_lnt(ctx, m.logl, d_lnt, nullptr, N, fd[0], fd[1], fd[2], fd[3], fd[4], fd[5]));
     B2N_TIME_END(ctx);
 
     const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;

@@ -434,7 +434,9 @@ int post_check(int64_t N, int n, int R, const double* x, int nq, const double* q
 extern "C" int b2n_weighted_stats(b2n_ctx* ctx, const double* x, int64_t N, int32_t n, const double* w, int32_t R,
                                   const double* shift, const double* q, int32_t nq, double* mean, double* cov,
                                   double* quant) {
-    if (!ctx || !w || !shift) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    B2N_TRY(b2n_refuse_reweight(ctx, "b2n_weighted_stats"));
+    if (!w || !shift) return B2N_ERR_ARG;
     B2N_TRY(post_check(N, n, R, x, nq, q, quant));
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     PostJob J;
@@ -521,12 +523,15 @@ extern "C" int b2n_jitter_posterior(b2n_ctx* ctx, const double* logl, const int6
                                     uint64_t chain0, const double* x, int32_t n, const double* q, int32_t nq,
                                     double* logz, double* logzerr, double* h, double* kld, double* mean, double* cov,
                                     double* quant) {
-    if (!ctx || !logl || !samples_n || !logwt_ref) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    const double* logrwt;
+    B2N_TRY(b2n_take_reweight(ctx, N, &logrwt));
+    if (!logl || !samples_n || !logwt_ref) return B2N_ERR_ARG;
     B2N_TRY(post_check(N, n, R, x, nq, q, quant));
     return post_realisations(ctx, N, x, n, R, q, nq, logz, logzerr, h, kld, mean, cov, quant,
                              [&](double* const sum[4], double* W, const double** w2, int64_t* nw2, const double** wref) {
                                  return b2n_jitter_produce(ctx, logl, samples_n, N, logwt_ref, logz_ref, approx, R,
-                                                           seed, chain0, sum, nullptr, W, w2, nw2, wref);
+                                                           seed, chain0, logrwt, sum, nullptr, W, w2, nw2, wref);
                              });
 }
 
@@ -536,12 +541,15 @@ extern "C" int b2n_resample_posterior(b2n_ctx* ctx, const double* logl, const in
                                       uint64_t seed, uint64_t chain0, const double* x, int32_t n, const double* q,
                                       int32_t nq, double* logz, double* logzerr, double* h, double* kld, double* mean,
                                       double* cov, double* quant) {
-    if (!ctx || !logl || !strand || !base || !piece_ptr || !logwt_ref || S < 1) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    const double* logrwt;
+    B2N_TRY(b2n_take_reweight(ctx, N, &logrwt));
+    if (!logl || !strand || !base || !piece_ptr || !logwt_ref || S < 1) return B2N_ERR_ARG;
     B2N_TRY(post_check(N, n, R, x, nq, q, quant));
     return post_realisations(ctx, N, x, n, R, q, nq, logz, logzerr, h, kld, mean, cov, quant,
                              [&](double* const sum[4], double* W, const double** w2, int64_t* nw2, const double** wref) {
                                  return b2n_resample_produce(ctx, logl, strand, N, S, base, piece_ptr, piece_strand,
-                                                             end, logwt_ref, logz_ref, R, seed, chain0, sum, nullptr,
-                                                             W, w2, nw2, wref);
+                                                             end, logwt_ref, logz_ref, R, seed, chain0, logrwt, sum,
+                                                             nullptr, W, w2, nw2, wref);
                              });
 }

@@ -46,6 +46,7 @@ struct RArgs {
     double* w;                   // N x R (sample-major): W = sum over a sample's copies of exp(logwt - logz[-1]),
                                  // -0.0 for a sample not drawn (resample_weights_kernel only)
     double* w2;                  // R: sum over the copies of exp(logwt - logz[-1])^2 (resample_weights_kernel only)
+    const double* lrw;           // N: log-reweight added to the logwt of every copy (the _rw kernels only), else NULL
 };
 
 __global__ void __launch_bounds__(RS_BLOCK) resample_mult_kernel(RArgs A) {
@@ -72,8 +73,9 @@ __device__ __forceinline__ double copy_dlv(double n, int k, bool is_end) {
 }
 
 // WOUT: also the weights w / w2 (b2n_resample_posterior); resample_scan_kernel, without them, compiles to the code it
-// had before they existed.
-template <bool WOUT>
+// had before they existed.  RW: lrw of the sample is added to the logwt of each of its copies (the h increments keep the
+// unreweighted L and ldv2, as compute_integrals(reweight=) does); a KL term of zero weight is 0.
+template <bool WOUT, bool RW = false>
 __device__ __forceinline__ void resample_scan(const RArgs& A) {
     __shared__ double xc[RS_TILE], xp[RS_TILE], xv[RS_TILE], xz[RS_TILE], wsum[32];
     const int r = blockIdx.x;
@@ -124,7 +126,8 @@ __device__ __forceinline__ void resample_scan(const RArgs& A) {
                     double lv = c_lv + (q > 0 ? xv[q - 1] : 0.0);
                     for (int k = 0; k < mi; k++) {
                         const double d = copy_dlv(n, k, ie);
-                        const double w = lae(l, lp) + lv + log1p(-exp(d)) + ln_half;
+                        double w = lae(l, lp) + lv + log1p(-exp(d)) + ln_half;
+                        if (RW) w += A.lrw[i];
                         E = lae(E, w);
                         lv += d;
                         lp = l;
@@ -153,7 +156,8 @@ __device__ __forceinline__ void resample_scan(const RArgs& A) {
                     for (int k = 0; k < mi; k++) {
                         const double d = copy_dlv(n, k, ie);
                         const double ldv2 = lv + log1p(-exp(d)) + ln_half;
-                        const double w = lae(l, lp) + ldv2;
+                        double w = lae(l, lp) + ldv2;
+                        if (RW) w += A.lrw[i];
                         const double zn = lae(z, w);
                         const double a = exp(l - zmax + ldv2) * l + exp(lp - zmax + ldv2) * lp;
                         const double dh = a - zmax * (exp(zn - zmax) - exp(z - zmax));
@@ -161,7 +165,7 @@ __device__ __forceinline__ void resample_scan(const RArgs& A) {
                         c_t += dh * -d;
                         if (A.wref) {
                             const double lp1 = w - zmax;
-                            k_t += exp(lp1) * (lp1 - lp2);
+                            if (!RW || w != -INFINITY) k_t += exp(lp1) * (lp1 - lp2);
                         }
                         if (WOUT) {
                             const double wc = exp(w - zmax);
@@ -205,14 +209,16 @@ __device__ __forceinline__ void resample_scan(const RArgs& A) {
 
 __global__ void __launch_bounds__(RS_BLOCK) resample_scan_kernel(RArgs A) { resample_scan<false>(A); }
 __global__ void __launch_bounds__(RS_BLOCK) resample_weights_kernel(RArgs A) { resample_scan<true>(A); }
+__global__ void __launch_bounds__(RS_BLOCK) resample_scan_rw_kernel(RArgs A) { resample_scan<false, true>(A); }
+__global__ void __launch_bounds__(RS_BLOCK) resample_weights_rw_kernel(RArgs A) { resample_scan<true, true>(A); }
 
 }  // namespace
 
 int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
                          const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand, const uint8_t* end,
                          const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed, uint64_t chain0,
-                         double* const sum[4], int32_t* mult, double* w, const double** w2, int64_t* nw2,
-                         const double** wref) {
+                         const double* logrwt, double* const sum[4], int32_t* mult, double* w, const double** w2,
+                         int64_t* nw2, const double** wref) {
     if (piece_ptr[0] != 0 || piece_ptr[N] < 0 || (piece_ptr[N] > 0 && !piece_strand)) return B2N_ERR_ARG;
     for (int64_t i = 0; i < N; i++)
         if (strand[i] < 0 || strand[i] >= S || piece_ptr[i + 1] < piece_ptr[i]) return B2N_ERR_ARG;
@@ -232,6 +238,8 @@ int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand
     A.logl = (const double*)p;
     B2N_TRY(b2n_in(ctx, ctx->in1, logwt_ref, logwt_ref ? (size_t)N * sizeof(double) : 0, &p));
     A.wref = (const double*)p;
+    B2N_TRY(b2n_in(ctx, ctx->work1, logrwt, logrwt ? (size_t)N * sizeof(double) : 0, &p));
+    A.lrw = (const double*)p;
     B2N_TRY(b2n_in_host(ctx, ctx->in2, strand, (size_t)N * sizeof(int32_t), &p));
     A.strand = (const int32_t*)p;
     B2N_TRY(b2n_in_host(ctx, ctx->in3, piece_ptr, (size_t)(N + 1) * sizeof(int64_t), &p));
@@ -265,8 +273,8 @@ int b2n_resample_produce(b2n_ctx* ctx, const double* logl, const int32_t* strand
     const dim3 grid((unsigned)((std::max(A.nbase, A.nadd) + RS_BLOCK - 1) / RS_BLOCK), (unsigned)R);
     resample_mult_kernel<<<grid, RS_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
-    if (w) resample_weights_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
-    else resample_scan_kernel<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
+    if (w) (A.lrw ? resample_weights_rw_kernel : resample_weights_kernel)<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
+    else (A.lrw ? resample_scan_rw_kernel : resample_scan_kernel)<<<R, RS_BLOCK, 0, ctx->stream>>>(A);
     B2N_LAUNCH_CHECK(ctx);
     return B2N_OK;
 }
@@ -276,7 +284,10 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
                                  const uint8_t* end, const double* logwt_ref, double logz_ref, int32_t R,
                                  uint64_t seed, uint64_t chain0, double* logz, double* logzerr, double* h,
                                  double* kld, int32_t* mult) {
-    if (!ctx || !logl || !strand || !base || !piece_ptr || N < 1 || S < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
+    if (!ctx) return B2N_ERR_ARG;
+    const double* logrwt;
+    B2N_TRY(b2n_take_reweight(ctx, N, &logrwt));
+    if (!logl || !strand || !base || !piece_ptr || N < 1 || S < 1 || R < 1 || R > 65535) return B2N_ERR_ARG;
     if (!logwt_ref && kld) return B2N_ERR_ARG;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t rb = (size_t)R * sizeof(double);
@@ -284,7 +295,7 @@ extern "C" int b2n_resample_runs(b2n_ctx* ctx, const double* logl, const int32_t
     B2N_TRY(O.bind(ctx));
     double* const d[4] = {(double*)O.dev[0], (double*)O.dev[1], (double*)O.dev[2], (double*)O.dev[3]};
     B2N_TRY(b2n_resample_produce(ctx, logl, strand, N, S, base, piece_ptr, piece_strand, end, logwt_ref, logz_ref, R,
-                                 seed, chain0, d, (int32_t*)O.dev[4], nullptr, nullptr, nullptr, nullptr));
+                                 seed, chain0, logrwt, d, (int32_t*)O.dev[4], nullptr, nullptr, nullptr, nullptr));
     B2N_TIME_END(ctx);
     B2N_TRY(O.done(ctx));
     return b2n_finish(ctx);

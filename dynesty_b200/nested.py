@@ -44,6 +44,11 @@ class Results(dict):
         return ("niter: %d\nncall: %d\neff(%%): %6.3f\nlogz: %6.3f +/- %6.3f" %
                 (self['niter'], self['ncall'], self['eff'], self['logz'][-1], self['logzerr'][-1]))
 
+    def importance_weights(self):
+        """The normalised importance weight of every sample (utils.py:886-893): exp(logwt - logz[-1]) / its sum."""
+        wt = np.exp(self['logwt'] - self['logz'][-1])
+        return wt / wt.sum()
+
     def posterior_moments(self):
         w = np.exp(self['logwt'] - self['logz'][-1])
         w /= w.sum()
@@ -52,14 +57,17 @@ class Results(dict):
         return mean, (d * w[:, None]).T @ d
 
 
-def _integrate(logl, logvol):
+def _integrate(logl, logvol, reweight=None):
     """Trapezoid evidence / information integrals over the dead-point sequence
-    (utils.py:1411-1467 compute_integrals, same quadrature)."""
+    (utils.py:1411-1467 compute_integrals, same quadrature); reweight: the log-reweight added to every logwt, as
+    compute_integrals(reweight=) does (h keeps the unreweighted likelihoods, normalised by the reweighted logz[-1])."""
     lpad = np.concatenate([[LOWL], logl])
     dlv = np.diff(logvol, prepend=0)
     logdvol = logvol - dlv + np.log1p(-np.exp(dlv))
     logdvol2 = logdvol + math.log(0.5)
     logwt = np.logaddexp(lpad[1:], lpad[:-1]) + logdvol2
+    if reweight is not None:
+        logwt = logwt + reweight
     logz = np.logaddexp.accumulate(logwt)
     zmax = logz[-1]
     h1 = np.cumsum(np.exp(lpad[1:] - zmax + logdvol2) * lpad[1:] +

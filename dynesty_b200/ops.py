@@ -586,6 +586,22 @@ def _strand_record(N, strand, base, piece_ptr, piece_strand, end):
     return strand, base, pp, ps, end
 
 
+def _logrwt(logrwt, N):
+    """A log-reweight as the C API takes it: N float64 values, none NaN or +inf (-inf: zero weight)."""
+    rw = f64(logrwt)
+    if rw.shape != (N,):
+        raise ValueError("logrwt must hold one value per sample (%d)" % N)
+    if np.isnan(rw).any() or np.isposinf(rw).any():
+        raise ValueError("logrwt holds NaN or +inf")
+    return rw
+
+
+def _set_reweight(ctx, rw):
+    """b2n_set_reweight for the C call that follows at once (None: nothing pending)."""
+    if rw is not None:
+        ctx.set_reweight(ptr(rw), len(rw))
+
+
 def _summaries(R, kl):
     """The per-realisation outputs logz, logzerr, h and, with kl, kld (R each)."""
     o = dict(logz=np.empty(R), logzerr=np.empty(R), h=np.empty(R))
@@ -595,19 +611,22 @@ def _summaries(R, kl):
 
 
 def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, arrays=False,
-                ctx=None):
+                logrwt=None, ctx=None):
     """R prior-volume realisations of one record (jitter_run / kld_error, utils.py:1317-1408, 1932-1997); realisation
     r draws from the B2N stream (seed, chain0 + r).  Returns dict(logz, logzerr, h[, kld]) with R values each (the
     last elements of the realisations' arrays) and, with arrays=True, logvol_arr, logwt_arr, logz_arr[, kld_arr]
-    (R x N).  kld needs the input run's weights: logwt_ref (N) and logz_ref (its logz[-1])."""
+    (R x N).  kld needs the input run's weights: logwt_ref (N) and logz_ref (its logz[-1]).  logrwt (N): a log-reweight
+    added to every logwt of every realisation (b2n_set_reweight)."""
     ctx = _ctx(ctx)
     kl = logwt_ref is not None
     logl, n, wref = _jitter_record(logl, samples_n, logwt_ref, kl)
     N, R = len(logl), int(R)
+    rw = None if logrwt is None else _logrwt(logrwt, N)
     o = _summaries(R, kl)
     if arrays:
         for k in ('logvol', 'logwt', 'logz') + (('kld',) if kl else ()):
             o[k + '_arr'] = np.empty((R, N))
+    _set_reweight(ctx, rw)
     ctx.check(ctx.lib.b2n_jitter_runs(ctx.h, ptr(logl), ptr(n), N, ptr(wref), float(logz_ref) if kl else 0.0,
                                       int(bool(approx)), R, int(seed), int(chain0), ptr(o['logz']),
                                       ptr(o['logzerr']), ptr(o['h']), ptr(o.get('kld')), ptr(o.get('logvol_arr')),
@@ -616,13 +635,14 @@ def jitter_runs(logl, samples_n, R, seed, chain0=0, approx=False, logwt_ref=None
 
 
 def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, chain0=0, logwt_ref=None, logz_ref=None,
-                  multiplicities=False, ctx=None):
+                  multiplicities=False, logrwt=None, ctx=None):
     """R bootstrap realisations of one strand-labelled record (resample_run / kld_error(error='resample'),
     utils.py:1495-1660, 1932-1997); realisation r draws from the B2N stream (seed, chain0 + r).  strand: compacted
     strand index per sample (0..S-1); base: per strand, drawn in the base event; piece_ptr / piece_strand: CSR of
     the pieces whose first covered sample is i; end: per sample, the copies of a final live point share out its live
     count (or None).  Returns dict(logz, logzerr, h[, kld]) with R values each and, with multiplicities=True, mult
-    (R x S, int64): the times every strand is drawn."""
+    (R x S, int64): the times every strand is drawn.  logrwt (N): a log-reweight added to the logwt of every copy of
+    every sample (b2n_set_reweight)."""
     ctx = _ctx(ctx)
     logl = f64(logl)
     N = len(logl)
@@ -630,8 +650,10 @@ def resample_runs(logl, strand, base, piece_ptr, piece_strand, end, R, seed, cha
     S, R = len(base), int(R)
     kl = logwt_ref is not None
     wref = _logwt_ref(logwt_ref, N) if kl else None
+    rw = None if logrwt is None else _logrwt(logrwt, N)
     o = _summaries(R, kl)
     m = np.empty((R, S), dtype=np.int32) if multiplicities else None
+    _set_reweight(ctx, rw)
     ctx.check(ctx.lib.b2n_resample_runs(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps), ptr(end),
                                         ptr(wref), float(logz_ref) if kl else 0.0, R, int(seed), int(chain0),
                                         ptr(o['logz']), ptr(o['logzerr']), ptr(o['h']), ptr(o.get('kld')), ptr(m)))
@@ -687,16 +709,19 @@ def weighted_stats(x, w, shift, q=None, moments=True, ctx=None):
 
 
 def jitter_posterior(logl, samples_n, x, R, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, q=None,
-                     ctx=None):
+                     logrwt=None, ctx=None):
     """jitter_runs plus, per realisation, the weighted mean (R x n), covariance (R x n x n) and, with q, quantiles
-    (R x n x nq) of the sample positions x (N x n).  logwt_ref / logz_ref (the record's own) are required."""
+    (R x n x nq) of the sample positions x (N x n).  logwt_ref / logz_ref (the record's own) are required.  logrwt:
+    as in jitter_runs."""
     ctx = _ctx(ctx)
     logl, n_, wref = _jitter_record(logl, samples_n, logwt_ref, True)
     N, R = len(logl), int(R)
     x = _post_x(x, N)
     q = _post_q(q)
+    rw = None if logrwt is None else _logrwt(logrwt, N)
     o = _summaries(R, True)
     o.update(_post_outputs(R, x.shape[1], q, True))
+    _set_reweight(ctx, rw)
     ctx.check(ctx.lib.b2n_jitter_posterior(ctx.h, ptr(logl), ptr(n_), N, ptr(wref), float(logz_ref),
                                            int(bool(approx)), R, int(seed), int(chain0), ptr(x), x.shape[1], ptr(q),
                                            0 if q is None else len(q), ptr(o['logz']), ptr(o['logzerr']), ptr(o['h']),
@@ -705,9 +730,10 @@ def jitter_posterior(logl, samples_n, x, R, seed, chain0=0, approx=False, logwt_
 
 
 def resample_posterior(logl, strand, base, piece_ptr, piece_strand, end, x, R, seed, chain0=0, logwt_ref=None,
-                       logz_ref=None, q=None, ctx=None):
+                       logz_ref=None, q=None, logrwt=None, ctx=None):
     """resample_runs plus, per realisation, the weighted mean, covariance and, with q, quantiles of the sample
-    positions x (N x n) over the realisation's copies.  logwt_ref / logz_ref (the record's own) are required."""
+    positions x (N x n) over the realisation's copies.  logwt_ref / logz_ref (the record's own) are required.  logrwt:
+    as in resample_runs."""
     ctx = _ctx(ctx)
     logl = f64(logl)
     N = len(logl)
@@ -716,8 +742,10 @@ def resample_posterior(logl, strand, base, piece_ptr, piece_strand, end, x, R, s
     wref = _logwt_ref(logwt_ref, N)
     x = _post_x(x, N)
     q = _post_q(q)
+    rw = None if logrwt is None else _logrwt(logrwt, N)
     o = _summaries(R, True)
     o.update(_post_outputs(R, x.shape[1], q, True))
+    _set_reweight(ctx, rw)
     ctx.check(ctx.lib.b2n_resample_posterior(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps),
                                              ptr(end), ptr(wref), float(logz_ref), R, int(seed), int(chain0), ptr(x),
                                              x.shape[1], ptr(q), 0 if q is None else len(q), ptr(o['logz']),
@@ -766,4 +794,20 @@ def merge_runs(logl, samples_n, run_ptr, nbase, lowedge=None, arrays=True, ctx=N
                                      ptr(o['samples_n']), ptr(last), ptr(o.get('logvol')), ptr(o.get('logwt')),
                                      ptr(o.get('logz')), ptr(o.get('logzvar')), ptr(o.get('h'))))
     o.update(logz_end=float(last[0]), logzerr_end=float(last[1]), h_end=float(last[2]))
+    return o
+
+
+def compute_integrals(logl, logvol, logrwt=None, ctx=None):
+    """compute_integrals(logl, logvol, reweight=logrwt) (utils.py:1411-1467; include/b200nest.h,
+    b2n_compute_integrals) on the GPU.  Returns dict(logwt, logz, logzvar, h) (N each)."""
+    logl = f64(logl)
+    N = len(logl)
+    logvol = f64(logvol)
+    if logl.ndim != 1 or N < 1 or logvol.shape != (N,):
+        raise ValueError("logl and logvol must be 1-D arrays of the same, non-zero length")
+    rw = None if logrwt is None else _logrwt(logrwt, N)
+    o = {k: np.empty(N) for k in ('logwt', 'logz', 'logzvar', 'h')}
+    ctx = _ctx(ctx)
+    ctx.check(ctx.lib.b2n_compute_integrals(ctx.h, ptr(logl), ptr(logvol), ptr(rw), N, None, ptr(o['logwt']),
+                                            ptr(o['logz']), ptr(o['logzvar']), ptr(o['h'])))
     return o

@@ -8,6 +8,7 @@ What is mirrored (reference py/dynesty/utils.py, same names / meaning):
   merge_runs    :1817-1929   several runs merged into one (``b2n_merge_runs``)
   mean_and_cov  :1081-1117   weighted mean and covariance (``b2n_weighted_stats``)
   quantile      :1196-1233   weighted quantiles (``b2n_weighted_stats``; unweighted: np.percentile)
+  reweight_run  :1663-1708   a run's weights for a new target (``b2n_compute_integrals``)
 and the batched forms the dynamic sampler's stopping function needs: ``jitter_realisations`` (``b2n_jitter_runs``) and
 ``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches,
 and ``posterior_realisations``: the same realisations with the posterior mean, covariance and quantiles of each
@@ -16,6 +17,11 @@ and ``posterior_realisations``: the same realisations with the posterior mean, c
 Randomness: realisation r of a call is the B2N Philox stream (seed, chain0 + r) (include/b200nest.h), so a (seed,
 chain) pair names one realisation: it is the same whether it is computed alone or in a batch of any size.
 ``seed=None`` draws a fresh seed, like the reference's ``rstate=None``.
+
+A record that ``reweight_run`` made carries its log-reweight as ``logrwt`` (N).  Every realisation of it -- jitter,
+resample, posterior, kld_error -- then carries that reweight too (``b2n_set_reweight``), so the reweighted evidence and
+posterior get the same error bars the original target has; the reference's realisations drop it.  ``merge_runs``
+refuses such records: the reweight is per sample, so merge first, then reweight.
 
 Strands need a record with samples_id / samples_it (``run_nested(strands=True)``).  The live count of a resampled
 point follows the strand rule of include/b200nest.h (b2n_resample_runs, DESIGN.md section 15): every point is live
@@ -47,6 +53,16 @@ def samples_n_of(res):
     raise ValueError("Final number of samples differs from number of iterations and number of live points.")
 
 
+def _logrwt(res):
+    """The record's log-reweight (reweight_run), or None."""
+    return np.asarray(res['logrwt'], dtype=float) if 'logrwt' in res else None
+
+
+def _rw(res):
+    """The ops keyword of the record's log-reweight: none for a record without one, which is called as before."""
+    return {} if 'logrwt' not in res else dict(logrwt=_logrwt(res))
+
+
 def _logz_end(res):
     """The record's own logz[-1] (the reference weights' normalisation)."""
     return float(np.asarray(res['logz'])[-1])
@@ -57,7 +73,8 @@ def jitter_realisations(res, n_mc, seed, chain0=0, approx=False, arrays=False, c
     realisation's logz / logzerr / information / cumulative KL divergence (n_mc values each); with arrays=True also
     logvol_arr, logwt_arr, logz_arr, kld_arr (n_mc x nsamps).  Realisation r uses the stream (seed, chain0 + r)."""
     return ops.jitter_runs(res['logl'], samples_n_of(res), int(n_mc), int(seed), chain0=int(chain0),
-                           approx=approx, logwt_ref=res['logwt'], logz_ref=_logz_end(res), arrays=arrays, ctx=ctx)
+                           approx=approx, logwt_ref=res['logwt'], logz_ref=_logz_end(res), arrays=arrays,
+                           ctx=ctx, **_rw(res))
 
 
 def _realisation(res, seed, chain, approx, ctx):
@@ -65,7 +82,7 @@ def _realisation(res, seed, chain, approx, ctx):
     logvol = o['logvol_arr'][0]
     # logzerr and information as arrays: the quadrature of compute_integrals on the realisation's volumes (host,
     # O(nsamps) for the one realisation; their last elements are the kernel's)
-    _, _, logzvar, h = _integrate(np.asarray(res['logl'], dtype=float), logvol)
+    _, _, logzvar, h = _integrate(np.asarray(res['logl'], dtype=float), logvol, reweight=_logrwt(res))
     new = Results(res)
     new.update(logvol=logvol, logwt=o['logwt_arr'][0], logz=o['logz_arr'][0],
                logzerr=np.sqrt(np.maximum(logzvar, 0)), information=h)
@@ -87,7 +104,8 @@ def kld_error(res, error='jitter', seed=None, chain=0, return_new=False, approx=
         new, idx = resample_run(res, seed, chain, return_idx=True, ctx=ctx)
         logp2 = (np.asarray(res['logwt']) - np.asarray(res['logz'])[-1])[idx]
         logp1 = new['logwt'] - new['logz'][-1]
-        kld = np.cumsum(np.exp(logp1) * (logp1 - logp2))
+        with np.errstate(invalid='ignore'):            # a term of zero weight (a -inf reweight) is 0
+            kld = np.cumsum(np.where(logp1 == -np.inf, 0.0, np.exp(logp1) * (logp1 - logp2)))
         return (kld, new) if return_new else kld
     if error != 'jitter':
         raise ValueError("Input `'error'` option '{}' is not valid.".format(error))
@@ -186,7 +204,7 @@ def resample_realisations(res, n_mc, seed, chain0=0, multiplicities=False, ctx=N
     drawn.  Realisation r uses the stream (seed, chain0 + r)."""
     rec = _strand_inputs(res)[1]
     return ops.resample_runs(*rec, int(n_mc), int(seed), chain0=int(chain0), logwt_ref=res['logwt'],
-                             logz_ref=_logz_end(res), multiplicities=multiplicities, ctx=ctx)
+                             logz_ref=_logz_end(res), multiplicities=multiplicities, ctx=ctx, **_rw(res))
 
 
 def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
@@ -211,13 +229,14 @@ def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
     samp_n = n[idx] - (0 if plan['end'] is None else copy * plan['end'][idx])     # a final live point's copies
     logvol = np.cumsum(np.log(samp_n / (samp_n + 1.)))
     lnew = logl[idx]
-    logwt, logz, logzvar, h = _integrate(lnew, logvol)
+    rw = _logrwt(res)
+    logwt, logz, logzvar, h = _integrate(lnew, logvol, reweight=None if rw is None else rw[idx])
     new = Results(res)
     nc = np.asarray(res['ncall_per_it'])[idx]
     new.update(niter=len(idx), ncall_per_it=nc, eff=100. * len(idx) / max(int(nc.sum()), 1), logl=lnew,
                samples_n=samp_n, logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(np.maximum(logzvar, 0)),
                information=h)
-    for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'samples_scale'):
+    for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'samples_scale', 'logrwt'):
         if k in res and len(res[k]) == N:
             new[k] = np.asarray(res[k])[idx]
     return (new, idx) if return_idx else new
@@ -230,6 +249,7 @@ def unravel_run(res):
     ids = np.asarray(res['samples_id'])
     added_live = plan['end'] is not None
     logl_all = np.asarray(res['logl'], dtype=float)
+    rw_all = _logrwt(res)
     out = []
     for s in plan['ids']:
         sel = ids == s
@@ -239,11 +259,11 @@ def unravel_run(res):
         logvol = -math.log(2) * (1. + np.arange(niter))
         if added_live:
             logvol = np.append(logvol, (logvol[-1] if niter else 0.0) + math.log(0.5))
-        logwt, logz, logzvar, h = _integrate(logl, logvol)
+        logwt, logz, logzvar, h = _integrate(logl, logvol, reweight=None if rw_all is None else rw_all[sel])
         nc = np.asarray(res['ncall_per_it'])[sel]
         r = Results(nlive=1, niter=niter, ncall_per_it=nc, eff=100. * nsamps / max(int(nc.sum()), 1), logl=logl,
                     logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(logzvar), information=h)
-        for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch'):
+        for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'logrwt'):
             if k in res and len(res[k]) == len(ids):
                 r[k] = np.asarray(res[k])[sel]
         if 'batch_bounds' in res:
@@ -306,9 +326,10 @@ def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=Fal
     logz_ref = _logz_end(res)
     if error == 'jitter':
         return ops.jitter_posterior(logl, samples_n_of(res), x, int(n_mc), int(seed), chain0=int(chain0),
-                                    approx=approx, logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx)
+                                    approx=approx, logwt_ref=res['logwt'], logz_ref=logz_ref, q=q,
+                                    ctx=ctx, **_rw(res))
     return ops.resample_posterior(*_strand_inputs(res)[1], x, int(n_mc), int(seed), chain0=int(chain0),
-                                  logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx)
+                                  logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx, **_rw(res))
 
 
 # ---------------------------------------------------------------------------------------------- merging runs
@@ -381,6 +402,9 @@ def merge_runs(res_list, ctx=None):
         NotImplementedError on the merged run.
     A single run is returned as it is (after check_result_static), as the reference does."""
     res_list = list(res_list)
+    if any('logrwt' in r for r in res_list):
+        raise ValueError("merge_runs: a run carries a log-reweight (reweight_run); the reweight is per sample, so "
+                         "merge first, then reweight")
     order, nbase = merge_order(res_list)
     ndims = {np.shape(r[k])[1] for r in res_list for k in ('samples_u', 'samples') if k in r and np.ndim(r[k]) == 2}
     if len(ndims) > 1:
@@ -432,3 +456,41 @@ def merge_runs(res_list, ctx=None):
             off += int(i.max()) + 1
         new.update(samples_id=np.concatenate(ids)[perm], samples_it=gather('samples_it').astype(np.int64))
     return check_result_static(new)
+
+
+# ---------------------------------------------------------------------------------------------- importance reweighting
+def reweight_run(res, logp_new=None, logp_old=None, model=None, ctx=None):
+    """reweight_run (utils.py:1663-1708): a copy of `res` whose weights are those of a new target, without rerunning.
+    logrwt = logp_new - logp_old (logp_old: res['logl'] when not given), and compute_integrals(logl, logvol,
+    reweight=logrwt) on the GPU (``b2n_compute_integrals``) gives logwt, logz and logzerr = sqrt(max(logzvar, 0)).
+    Give exactly one of logp_new (N) and model: a ``DeviceModel`` whose likelihood is evaluated at every res['samples']
+    in one launch (its likelihood-only twin, the model id ids()[1]).  logrwt may hold -inf (zero weight), not NaN or
+    +inf, and not -inf everywhere.  The copy keeps logvol and records logrwt (N), which the realisations of this
+    module carry from then on.  As in the reference, `information` is the input's: the reference hands h over under
+    the key 'h', which its Results drops."""
+    if (logp_new is None) == (model is None):
+        raise ValueError("reweight_run needs exactly one of logp_new and model")
+    logl = np.asarray(res['logl'], dtype=float)
+    N = len(logl)
+    if model is not None:
+        x = np.asarray(res['samples']) if 'samples' in res else np.empty((0, 0))
+        if x.ndim != 2 or len(x) != N or x.shape[1] < 1:
+            raise ValueError("reweight_run(model=) needs the sample positions of every point (res['samples']); a run "
+                             "made with keep_samples=False has none")
+        if x.shape[1] != model.ndim:
+            raise ValueError("the model has %d dimensions, the samples %d" % (model.ndim, x.shape[1]))
+        logp_new = ops.model_eval(model.ids(ctx)[1], x, want_v=False, ctx=ctx)[1]
+    logp_new = np.asarray(logp_new, dtype=float)
+    logp_old = logl if logp_old is None else np.asarray(logp_old, dtype=float)
+    if logp_new.shape != (N,) or logp_old.shape != (N,):
+        raise ValueError("logp_new and logp_old must hold one value per sample (%d)" % N)
+    with np.errstate(invalid='ignore'):
+        logrwt = logp_new - logp_old
+    if np.isnan(logrwt).any() or np.isposinf(logrwt).any():
+        raise ValueError("logp_new - logp_old holds NaN or +inf")
+    if np.all(logrwt == -np.inf):
+        raise ValueError("logp_new - logp_old is -inf at every sample: the new target gives the run no weight")
+    o = ops.compute_integrals(logl, res['logvol'], logrwt, ctx=ctx)
+    new = Results(res)
+    new.update(logwt=o['logwt'], logz=o['logz'], logzerr=np.sqrt(np.maximum(o['logzvar'], 0)), logrwt=logrwt)
+    return new

@@ -441,6 +441,31 @@ int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, c
                    int32_t nbase, const double* lowedge, int64_t* perm, int64_t* samples_n_out, double* last3,
                    double* logvol, double* logwt, double* logz, double* logzvar, double* h);
 
+/* ---- importance reweighting (reweight_run, utils.py:1663-1708; compute_integrals(reweight=), :1411-1467) ----------
+ * A log-reweight logrwt_i = logp_new_i - logp_old_i per sample changes one thing in the quadrature: for every sample,
+ * or every copy of a sample in a resample realisation,
+ *   logwt_i = logaddexp(L_i, L_{i-1}) + logdvol2_i + logrwt_i.
+ * logz, the importance weights exp(logwt - logz[-1]) and the KL terms p1 (ln p1 - ln p2), ln p1 = logwt - logz[-1],
+ * follow from it.  The h increments exp(L - zmax + logdvol2) L + .. keep the UNREWEIGHTED L and logdvol2, normalised by
+ * the reweighted zmax = logz[-1], so h and logzvar are those of the reference's compute_integrals(reweight=).  Entries
+ * may be -inf (zero weight: a KL term of zero weight is 0, where the reference would compute 0 * -inf = NaN); NaN and
+ * +inf are refused in host-pointer mode and undefined in device-pointer mode.
+ *
+ * b2n_compute_integrals: compute_integrals(logl, logvol, reweight=logrwt) of one record on the deterministic passes of
+ * b2n_jitter_runs (ln t = diff(logvol, prepend=0)).  logrwt may be NULL (no reweight).  logl, logvol, logrwt: N, host
+ * or device like the outputs.  Outputs, each may be NULL: last3 (3): logz[-1], logzerr[-1] = sqrt(|logzvar[-1]|),
+ * h[-1]; logwt, logz, logzvar, h (N each).  FP64, sums reassociated (block scans).  5 or 6 kernel launches (6 when
+ * logzvar or h is asked for).  Synchronises in host-pointer mode. */
+int b2n_compute_integrals(b2n_ctx* ctx, const double* logl, const double* logvol, const double* logrwt, int64_t N,
+                          double* last3, double* logwt, double* logz, double* logzvar, double* h);
+/* b2n_set_reweight: the log-reweight (N, host or device like the arrays of the call) for the NEXT b2n_jitter_runs /
+ * b2n_resample_runs / b2n_jitter_posterior / b2n_resample_posterior call, whose realisations then carry it as above
+ * (one call, then reset, however that call ends; the array must stay valid until then).  That call needs the same N,
+ * else it fails with B2N_ERR_ARG.  b2n_merge_runs, b2n_weighted_stats and b2n_compute_integrals called with a
+ * reweight pending clear it and return B2N_ERR_UNSUPPORTED.  NULL cancels.  The realisation entry points keep their
+ * launch counts; with the reweight they run the _rw instantiations of the same passes. */
+int b2n_set_reweight(b2n_ctx* ctx, const double* logrwt, int64_t N);
+
 /* ---- resident bound for the proposal kernels --------------------------------
  * Uploads K ellipsoids of dimension ncdim (what Sampler ships to every task as
  * `axes` / kwargs['bound'], sampler.py:708-717, internal_samplers.py:229-233).
