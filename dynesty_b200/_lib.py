@@ -88,6 +88,7 @@ SYMBOLS = {
     'b2n_last_kernel_ms': (C.c_double, [_P]),
     'b2n_model_create': (C.c_int, [_P, C.POINTER(ModelDesc), C.POINTER(_I)]),
     'b2n_model_eval': (C.c_int, [_P, _I, _P, _L, _P, _P]),
+    'b2n_model_blob': (C.c_int, [_P, _I, _P, _L, _I, _P]),
     'b2n_user_kernel_exprs': (C.c_int, [C.POINTER(C.POINTER(C.c_char_p)), C.POINTER(_I)]),
     'b2n_model_create_user': (C.c_int, [_P, C.POINTER(ModelDesc), _P, _L, _P, C.c_size_t, C.POINTER(C.c_char_p),
                                         C.POINTER(_I)]),

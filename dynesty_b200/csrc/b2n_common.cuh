@@ -148,6 +148,8 @@ struct b2n_ctx {
     // B2nUserSlot (empty for a registry model); the libraries are unloaded by b2n_free
     std::vector<std::vector<const void*>> user_fn;
     std::vector<cudaLibrary_t> user_libs;
+    // user_blob[model id]: the image's b2n_user_blob_kernel (b2n_model_blob), NULL for a model without blobs
+    std::vector<const void*> user_blob;
 };
 
 // The kernel instantiations a user likelihood is compiled into, in the order of b2n_user_kernel_exprs (b2n_ctx.cu).

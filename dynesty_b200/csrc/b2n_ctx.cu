@@ -122,6 +122,8 @@ void b2n_free(b2n_ctx* ctx) {
     for (void* p : ctx->model_allocs) cudaFree(p);
     for (const auto& fns : ctx->user_fn)
         for (const void* f : fns) b2n_func_smem_forget(ctx->device, f);
+    for (const void* f : ctx->user_blob)
+        if (f) b2n_func_smem_forget(ctx->device, f);
     for (cudaLibrary_t l : ctx->user_libs) cudaLibraryUnload(l);
     if (ctx->ev0) { cudaEventDestroy(ctx->ev0); cudaEventDestroy(ctx->ev1); }
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
@@ -263,6 +265,7 @@ int b2n_model_create(b2n_ctx* ctx, const b2n_model_desc* d, int32_t* id) {
     B2N_TRY(upload(ctx, d->like_mat, n * n, &m.lmat));
     ctx->models.push_back(m);
     ctx->user_fn.emplace_back();
+    ctx->user_blob.push_back(nullptr);
     *id = (int32_t)ctx->models.size() - 1;
     return B2N_OK;
 }
@@ -341,6 +344,12 @@ static int model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double
         }
         fns[s] = (const void*)k;
     }
+    // the blob kernel is there only when the program was compiled with B2N_USER_BLOB; without it the model has no blob
+    cudaKernel_t blob_k = nullptr;
+    if (cudaLibraryGetKernel(&blob_k, lib, "b2n_user_blob_kernel") != cudaSuccess) {
+        cudaGetLastError();              // (not sticky: the context stays usable)
+        blob_k = nullptr;
+    }
     const size_t n = d->ndim;
     B2nModel m;
     memset(&m, 0, sizeof(m));
@@ -356,6 +365,7 @@ static int model_create_user(b2n_ctx* ctx, const b2n_model_desc* d, const double
     B2N_TRY(upload_padded(ctx, params, nparams, n, &m.lv0));
     ctx->models.push_back(m);
     ctx->user_fn.push_back(fns);
+    ctx->user_blob.push_back((const void*)blob_k);
     *id = (int32_t)ctx->models.size() - 1;
     return B2N_OK;
 }
@@ -480,5 +490,48 @@ extern "C" int b2n_model_eval(b2n_ctx* ctx, int32_t id, const double* u, int64_t
     B2N_LAUNCH_CHECK(ctx);
     B2N_TRY(b2n_out_done(ctx, v, dv, M * n * sizeof(double)));
     B2N_TRY(b2n_out_done(ctx, logl, dl, M * sizeof(double)));
+    return b2n_finish(ctx);
+}
+
+extern "C" int b2n_model_blob(b2n_ctx* ctx, int32_t id, const double* v, int64_t M, int32_t nblob, double* blob) {
+    if (!ctx) return B2N_ERR_ARG;
+    if (id < 0 || id >= (int)ctx->models.size())
+        return b2n_fail(ctx, B2N_ERR_ARG, "b2n_model_blob: no such model");
+    if (ctx->models[id].like_kind != B2N_LIKE_USER)
+        return b2n_fail(ctx, B2N_ERR_ARG, "b2n_model_blob: a registry model has no blob (user models only)");
+    const void* f = ctx->user_blob[id];
+    if (!f)
+        return b2n_fail(ctx, B2N_ERR_ARG, "b2n_model_blob: the model's image has no b2n_user_blob_kernel (compile "
+                                          "b2n_user_blob with B2N_USER_BLOB defined)");
+    if (nblob < 1 || M < 0 || (M > 0 && (!v || !blob)))
+        return b2n_fail(ctx, B2N_ERR_ARG, "b2n_model_blob: needs nblob >= 1, M >= 0 and, for M > 0, v and blob");
+    const B2nModel m = ctx->models[id];
+    const size_t n = m.ndim;
+    // per warp: v, work and the blob row; as many warps per block (up to 8) as the opt-in limit holds
+    const size_t per_warp = (2 * n + (size_t)nblob) * sizeof(double);
+    if (per_warp > (size_t)ctx->max_smem_optin) {
+        snprintf(ctx->err, sizeof(ctx->err), "b2n_model_blob: %zu bytes of shared memory per point (2 ndim + nblob "
+                 "doubles) exceed the device's %d", per_warp, ctx->max_smem_optin);
+        return B2N_ERR_ARG;
+    }
+    if (M == 0) return B2N_OK;
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    const void* dv;
+    void* db;
+    B2N_TRY(b2n_in(ctx, ctx->in0, v, M * n * sizeof(double), &dv));
+    B2N_TRY(b2n_out(ctx, ctx->out0, blob, M * (size_t)nblob * sizeof(double), &db));
+    const int wpb = (int)std::min<size_t>(8, (size_t)ctx->max_smem_optin / per_warp);
+    const size_t smem = (size_t)wpb * per_warp;
+    int64_t blocks = (M + wpb - 1) / wpb;
+    if (blocks > (int64_t)ctx->sm_count * (64 / wpb)) blocks = (int64_t)ctx->sm_count * (64 / wpb);
+    B2N_TRY(b2n_func_smem(ctx, f, smem));
+    int64_t M_ = M;
+    int nb = nblob;
+    void* args[] = {(void*)&m, (void*)&dv, (void*)&M_, (void*)&nb, (void*)&db};
+    B2N_TIME_BEGIN(ctx);
+    B2N_CUDA(ctx, cudaLaunchKernel(f, dim3((unsigned)blocks), dim3(wpb * 32), args, smem, ctx->stream));
+    B2N_TIME_END(ctx);
+    B2N_LAUNCH_CHECK(ctx);
+    B2N_TRY(b2n_out_done(ctx, blob, db, M * (size_t)nblob * sizeof(double)));
     return b2n_finish(ctx);
 }

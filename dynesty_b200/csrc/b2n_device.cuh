@@ -103,6 +103,13 @@ __device__ __forceinline__ double region2d_logl(double shape, double x, double y
 __device__ double b2n_user_loglike(const double* v, double* work, int n, const double* p, int lane);
 #endif
 
+#ifdef B2N_USER_BLOB
+// the derived quantities of a point (contract: include/b200nest.h, b2n_model_blob), defined in the user's source;
+// only b2n_user_blob_kernel (b2n_user_kernels.cuh) calls it
+__device__ void b2n_user_blob(const double* v, double* work, int n, const double* p, int lane, double* blob,
+                              int nblob);
+#endif
+
 #ifdef B2N_USER_PRIOR
 // the user prior transform of a run-time compiled model (B2N_PRIOR_USER; contract: include/b200nest.h,
 // b2n_model_create_user_ex), defined after b2n_user_kernels.cuh in the same NVRTC program

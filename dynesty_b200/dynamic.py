@@ -133,7 +133,8 @@ def stopping_function(results, args=None, seed=None, chain0=0, return_vals=False
 
 
 def merge_two(saved, new, logl_min):
-    """combine_runs (dynamicsampler.py:1467-1608) for two records dict(u, v, logl, n, nc, scale, batch): both sorted
+    """combine_runs (dynamicsampler.py:1467-1608) for two records dict(u, v, logl, n, nc, scale, batch[, id, it, blob]),
+    every key one row per sample: both sorted
     by logl; ties go to the saved run; the live count of a merged point is its own run's plus -- above logl_min --
     the count the OTHER run has at that position."""
     ls, ln_ = saved['logl'], new['logl']
@@ -197,6 +198,8 @@ class DynamicNestedSampler:
         rec = dict(u=res['samples_u'], v=res['samples'], logl=res['logl'], n=np.asarray(res['samples_n'], dtype=np.int64),
                    nc=np.asarray(res['ncall_per_it'], dtype=np.int64), scale=np.asarray(res['samples_scale'], dtype=float),
                    batch=np.full(len(res['logl']), batch_id, dtype=np.int64))
+        if 'blob' in res:
+            rec['blob'] = np.asarray(res['blob'])
         if 'samples_id' in res:
             # a batch's strands are new strands: its slot ids follow the saved ones (dynamicsampler.py:1489)
             rec.update(id=np.asarray(res['samples_id'], dtype=np.int64) + id_offset,
@@ -213,6 +216,8 @@ class DynamicNestedSampler:
                                nbatch=self.batch)
         if 'id' in rec:
             self.results.update(samples_id=rec['id'], samples_it=rec['it'])
+        if 'blob' in rec:
+            self.results['blob'] = rec['blob']
         return self.results
 
     # ------------------------------------------------------------------ baseline (sample_initial, :927-1226)

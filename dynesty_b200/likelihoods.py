@@ -35,6 +35,7 @@ class DeviceModel:
         self.like_vec0, self.like_vec1 = opt(like_vec0, (n,)), opt(like_vec1, (n,))
         self.like_mat = opt(like_mat, (n, n))
         self.s = (float(s0), float(s1), float(s2))
+        self.nblob = 0          # doubles of derived quantities per point (from_cuda(nblob=)); registry models have none
         self._ids = {}          # ctx -> (full id, likelihood-only id)
 
     # -- pickling: device handles are per-process, re-created lazily ------------
@@ -53,7 +54,7 @@ class DeviceModel:
 
     @classmethod
     def from_cuda(cls, ndim, source, params=None, prior_kind=_lib.PRIOR_IDENTITY, prior_p0=None, prior_p1=None,
-                  prior_source=None, prior_params=None, name='user'):
+                  prior_source=None, prior_params=None, name='user', nblob=0):
         """A model whose log-likelihood (and optionally prior transform) is user CUDA code, compiled into the
         proposal kernels at run time.
 
@@ -121,12 +122,33 @@ class DeviceModel:
         ``prior_source`` excludes ``prior_kind`` / ``prior_p0`` / ``prior_p1``, and ``prior_params`` needs
         ``prior_source`` (``ValueError`` otherwise).  ``loglikelihood(v)`` stays prior-free.
 
+        With ``nblob > 0`` the model has a blob: ``nblob`` derived quantities per point, which the samplers save with
+        every sample (``NestedSampler(..., blob=True)``, ``results['blob']``).  ``source`` then also defines a third
+        warp-cooperative device function::
+
+            __device__ void b2n_user_blob(const double* v, double* work, int n, const double* p, int lane,
+                                          double* blob, int nblob);
+
+        * all 32 lanes call it; ``v`` (read only), ``work``, ``n``, ``p`` and ``lane`` are those of
+          ``b2n_user_loglike``, which it may call (a blob may hold the log-likelihood or its parts);
+        * ``blob``: ``nblob`` doubles of warp-private shared memory, NaN on entry; what it writes there is the point's
+          row of the blob, and an element it leaves unwritten stays NaN;
+        * the caller synchronises the warp before and after the call; inside it, ``__syncwarp()`` between one lane
+          writing ``work`` or ``blob`` and another reading it;
+        * it must be deterministic: the blob of a saved sample is computed from its ``v`` after the run, in one launch
+          (``blob(v)``), not carried through the chains.
+
+        A source without ``b2n_user_blob`` raises ``usermodel.UserModelCompileError`` naming it when the model is first
+        used.  ``blob(v)`` evaluates the blob of any points.
+
         The model is accepted wherever a registry model is: every sampler, the device-resident rounds, the dynamic
         sampler, replicas; random walks run on the warp-per-chain kernel.  The source is compiled with NVRTC for
         sm_90a (once per process, ``usermodel.compile_user``); a compile error raises
         ``usermodel.UserModelCompileError`` carrying NVRTC's log.  Pickling keeps ``source``, ``params``,
-        ``prior_source`` and ``prior_params``.
+        ``prior_source``, ``prior_params`` and ``nblob``.
         """
+        if isinstance(nblob, bool) or int(nblob) != nblob or nblob < 0:
+            raise ValueError('nblob must be a non-negative integer')
         if prior_source is not None:
             if prior_kind not in (_lib.PRIOR_IDENTITY, _lib.PRIOR_USER) or prior_p0 is not None or prior_p1 is not None:
                 raise ValueError('prior_source defines the prior: prior_kind / prior_p0 / prior_p1 do not apply')
@@ -140,6 +162,7 @@ class DeviceModel:
         m.params = None if params is None else f64(np.ravel(params))
         m.prior_source = None if prior_source is None else str(prior_source)
         m.prior_params = None if prior_params is None else f64(np.ravel(prior_params))
+        m.nblob = int(nblob)
         m.logz_truth = None
         return m
 
@@ -161,7 +184,7 @@ class DeviceModel:
     def _create_user(self, ctx, prior_kind, mid):
         from . import usermodel
         prior_source = getattr(self, 'prior_source', None)
-        cm = usermodel.compile_user(self.source, prior_source)
+        cm = usermodel.compile_user(self.source, prior_source, blob=getattr(self, 'nblob', 0) > 0)
         names = (C.c_char_p * len(cm.lowered))(*[s.encode() for s in cm.lowered])
         prm = self.params
         nprm = 0 if prm is None else prm.size
@@ -183,6 +206,15 @@ class DeviceModel:
         """(v, logl) of unit-cube points u (M, ndim) in one launch."""
         from . import ops
         return ops.model_eval(self.ids(ctx)[0], u, ctx=ctx)
+
+    def blob(self, v, ctx=None):
+        """The blob (M, nblob) of the physical points v (M, ndim) in one launch (``b2n_model_blob``)."""
+        from . import ops
+        if getattr(self, 'nblob', 0) < 1:
+            raise ValueError('the model %r has no blob: DeviceModel.from_cuda(..., nblob=k) with a source that '
+                             'defines b2n_user_blob' % self.name)
+        v = np.asarray(v, dtype=float).reshape(-1, self.ndim)
+        return ops.model_blob(self.ids(ctx)[0], v, self.nblob, ctx=ctx)
 
     def prior_transform(self, u):
         from . import ops

@@ -85,13 +85,22 @@ class NestedSampler:
     ``DeviceModel`` instead of the (loglikelihood, prior_transform) callables.
     `comm`: optional ``dynesty_b200.dist.Comm`` -- chains of a queue fill are sharded over
     the ranks and all-gathered (NCCL), every rank keeps the identical host state.
+    `live_points`: (u, v, logl), or the reference's (u, v, logl, blobs); the blobs are not read, because the blob of
+    every saved sample is computed from its v at the end of the run.
+    `blob`: save the model's blob with every sample, as ``results['blob']`` (nsamples x model.nblob).  It needs a
+    model with blobs (``DeviceModel.from_cuda(..., nblob=k)``).  The chains do not carry it: the blob is a
+    deterministic function of v, evaluated once per saved sample by one launch at the end of the run.
     """
 
     def __init__(self, model, nlive=500, bound='multi', sample='auto', ncdim=None, walks=None, slices=None,
                  facc=0.5, enlarge=None, bootstrap=None, update_interval=None, first_update=None,
                  queue_size=None, periodic=None, reflective=None, seed=56432, ctx=None, comm=None, live_points=None,
-                 live_init='device'):
+                 live_init='device', blob=False):
+        if blob and getattr(model, 'nblob', 0) < 1:
+            raise ValueError('blob=True needs a model with blobs: DeviceModel.from_cuda(..., nblob=k) with a source '
+                             'that defines b2n_user_blob')
         self.model = model
+        self.blob = bool(blob)
         self.ndim = n = model.ndim
         self.ncdim = ncdim or n
         self.nlive = int(nlive)
@@ -166,8 +175,8 @@ class NestedSampler:
         if comm is not None and self.queue_size % comm.world:
             self.queue_size += comm.world - self.queue_size % comm.world
         # -- live points (sampler.py:56-262, evaluated in one launch)
-        if live_points is not None:         # (u, v, logl) supplied by the caller (dynesty.py:600 `live_points`)
-            self.live_u, self.live_v, self.live_logl = (np.array(a, dtype=float) for a in live_points)
+        if live_points is not None:         # (u, v, logl[, blobs]) supplied by the caller (dynesty.py:600 `live_points`)
+            self.live_u, self.live_v, self.live_logl = (np.array(a, dtype=float) for a in live_points[:3])
         elif live_init == 'device':
             # _initialize_live_points (sampler.py:56-262) on the device: nlive prior draws + transform + likelihood in
             # ONE launch (b2n_unitcube_batch at threshold -inf: a draw whose logl is -inf is redrawn, the reference's
@@ -555,7 +564,7 @@ class NestedSampler:
         logl_max      : stop once the lowest live point is above it (sampler.py:1103-1106; the end of a dynamic batch).
         keep_samples  : loop='device' only.  False = the positions of the dead points are NOT brought back from the
                         device (results.samples / samples_u are then empty; logz, logzerr, logl, logvol, logwt and the
-                        call counts are complete): for ensembles that only want evidences.
+                        call counts are complete): for ensembles that only want evidences.  Not with blob=True.
         device_init   : False = the phase before the first bound runs in the host loop (queue of prior draws
                         evaluated on the GPU) and the device takes over when the first bound exists.
         strands       : True = record every sample's strand (the reference's samples_id / samples_it): the results
@@ -566,6 +575,9 @@ class NestedSampler:
             return self._resume(checkpoint_file, checkpoint_every)
         if loop not in ('host', 'device'):
             raise ValueError("loop must be 'host' or 'device'")
+        if self.blob and not keep_samples:
+            raise ValueError("blob=True needs the sample positions: the blobs are computed from them "
+                             "(keep_samples=False)")
         if checkpoint_file is not None and loop != 'device':
             raise ValueError("checkpointing is implemented for loop='device'")
         if loop == 'device' and self.comm is not None:
@@ -733,4 +745,6 @@ class NestedSampler:
             if add_live:
                 ids, its = np.concatenate([ids, order]), np.concatenate([its, self.live_it[order]])
             self.results.update(samples_id=ids.astype(np.int64), samples_it=its.astype(np.int64))
+        if getattr(self, 'blob', False):           # (a sampler pickled before blobs existed has no flag)
+            self.results['blob'] = self.model.blob(sv, ctx=self.ctx)
         return self.results

@@ -23,6 +23,16 @@ def model_eval(model, u, want_v=True, ctx=None):
     return v, logl
 
 
+def model_blob(model, v, nblob, ctx=None):
+    """The blob (M, nblob) of the physical points v (M, ndim) of a user model with blobs (b2n_model_blob)."""
+    ctx = _ctx(ctx)
+    v = f64(np.atleast_2d(v))
+    M = len(v)
+    blob = np.empty((M, int(nblob)))
+    ctx.check(ctx.lib.b2n_model_blob(ctx.h, model, ptr(v), M, int(nblob), ptr(blob)))
+    return blob
+
+
 def membership(x, ctrs, ams, strict=True, want_d2=False, ctx=None):
     """mask (M, K) bool, q (M,) int32 [, d2 (M, K)]  (bounding.py:502-523)."""
     ctx = _ctx(ctx)

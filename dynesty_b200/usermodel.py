@@ -1,14 +1,14 @@
 """Run-time compilation of user likelihoods (B2N_LIKE_USER) and user priors (B2N_PRIOR_USER) with NVRTC.
 
 The user writes one warp-cooperative CUDA device function ``b2n_user_loglike``, and optionally a second one,
-``b2n_user_prior`` (contract: ``include/b200nest.h``, ``DeviceModel.from_cuda``).  ``compile_user`` compiles the
-library's chain-kernel templates with them -- the program is ``b2n_user_kernels.cuh`` followed by the user's
-source -- for sm_90a, asking NVRTC for every instantiation the library lists (``b2n_user_kernel_exprs``), and
-returns the cubin and the mangled kernel names that ``b2n_model_create_user(_ex)`` loads.  No GPU is needed to
-compile.
+``b2n_user_prior``, and a third, ``b2n_user_blob`` (contract: ``include/b200nest.h``, ``DeviceModel.from_cuda``).
+``compile_user`` compiles the library's chain-kernel templates with them -- the program is ``b2n_user_kernels.cuh``
+followed by the user's source -- for sm_90a, asking NVRTC for every instantiation the library lists
+(``b2n_user_kernel_exprs``), and returns the cubin and the mangled kernel names that ``b2n_model_create_user(_ex)``
+loads.  No GPU is needed to compile.
 
-A compile is done once per process for a given (source, options) and kept in memory only: nothing is cached on
-disk, like the library build itself (build.py).
+A compile is done once per process for a given (source, prior, blob switch, options) and kept in memory only:
+nothing is cached on disk, like the library build itself (build.py).
 """
 import ctypes as C
 import glob
@@ -149,14 +149,17 @@ def kernel_exprs():
     return [arr[i].decode() for i in range(cnt.value)]
 
 
-def program_source(source, prior_source=None):
+def program_source(source, prior_source=None, blob=False):
     """The NVRTC program of a user likelihood: the kernel templates, then the user's code (line numbers of NVRTC
     messages refer to the user's source).  With a user prior (``prior_source`` defines b2n_user_prior) the
-    templates are compiled with B2N_USER_PRIOR, and the prior precedes the likelihood under its own file name."""
+    templates are compiled with B2N_USER_PRIOR, and the prior precedes the likelihood under its own file name.  With
+    blob=True (``source`` also defines b2n_user_blob) the program is compiled with B2N_USER_BLOB, which adds the
+    kernel b2n_user_blob_kernel."""
+    head = '#define B2N_USER_BLOB\n' if blob else ''
     if prior_source is None:
-        return '#include "b2n_user_kernels.cuh"\n#line 1 "user_likelihood.cu"\n' + source + '\n'
-    return ('#define B2N_USER_PRIOR\n#include "b2n_user_kernels.cuh"\n#line 1 "user_prior.cu"\n' + prior_source +
-            '\n#line 1 "user_likelihood.cu"\n' + source + '\n')
+        return head + '#include "b2n_user_kernels.cuh"\n#line 1 "user_likelihood.cu"\n' + source + '\n'
+    return ('#define B2N_USER_PRIOR\n' + head + '#include "b2n_user_kernels.cuh"\n#line 1 "user_prior.cu"\n' +
+            prior_source + '\n#line 1 "user_likelihood.cu"\n' + source + '\n')
 
 
 class CompiledUserModel:
@@ -164,18 +167,27 @@ class CompiledUserModel:
         self.cubin, self.exprs, self.lowered, self.log, self.seconds = cubin, exprs, lowered, log, seconds
 
 
-def compile_user(source, prior_source=None):
-    """Compile `source` (defines b2n_user_loglike) and, if given, `prior_source` (defines b2n_user_prior) into
-    every user-kernel slot; memoised per process."""
+def compile_user(source, prior_source=None, blob=False):
+    """Compile `source` (defines b2n_user_loglike, and with blob=True b2n_user_blob) and, if given, `prior_source`
+    (defines b2n_user_prior) into every user-kernel slot; memoised per process."""
     import time
     options = OPTIONS + tuple('-I' + d for d in [CSRC, INCLUDE] + cuda_include_dirs())
-    key = (source, options) if prior_source is None else (source, options, prior_source)
+    blob = bool(blob)
+    key = (source, options, prior_source, blob)
     with _mu:
         hit = _cache.get(key)
         if hit is None:
             exprs = kernel_exprs()
             t0 = time.perf_counter()
-            cubin, lowered, log = nvrtc().compile(program_source(source, prior_source), 'b2n_user_model.cu', exprs,
-                                                  list(options))
+            try:
+                cubin, lowered, log = nvrtc().compile(program_source(source, prior_source, blob), 'b2n_user_model.cu',
+                                                      exprs, list(options))
+            except UserModelCompileError as e:
+                if blob and 'b2n_user_blob' in str(e):
+                    raise UserModelCompileError(
+                        'a model with blobs (nblob > 0) needs its source to define __device__ void b2n_user_blob('
+                        'const double* v, double* work, int n, const double* p, int lane, double* blob, int nblob)'
+                        '\n' + str(e)) from None
+                raise
             hit = _cache[key] = CompiledUserModel(cubin, exprs, lowered, log, time.perf_counter() - t0)
         return hit

@@ -236,7 +236,7 @@ def resample_run(res, seed=None, chain=0, return_idx=False, ctx=None):
     new.update(niter=len(idx), ncall_per_it=nc, eff=100. * len(idx) / max(int(nc.sum()), 1), logl=lnew,
                samples_n=samp_n, logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(np.maximum(logzvar, 0)),
                information=h)
-    for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'samples_scale', 'logrwt'):
+    for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'samples_scale', 'logrwt', 'blob'):
         if k in res and len(res[k]) == N:
             new[k] = np.asarray(res[k])[idx]
     return (new, idx) if return_idx else new
@@ -263,7 +263,7 @@ def unravel_run(res):
         nc = np.asarray(res['ncall_per_it'])[sel]
         r = Results(nlive=1, niter=niter, ncall_per_it=nc, eff=100. * nsamps / max(int(nc.sum()), 1), logl=logl,
                     logvol=logvol, logwt=logwt, logz=logz, logzerr=np.sqrt(logzvar), information=h)
-        for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'logrwt'):
+        for k in ('samples', 'samples_u', 'samples_id', 'samples_it', 'samples_batch', 'logrwt', 'blob'):
             if k in res and len(res[k]) == len(ids):
                 r[k] = np.asarray(res[k])[sel]
         if 'batch_bounds' in res:
@@ -309,18 +309,24 @@ def quantile(x, q, weights=None, ctx=None):
     return o['quantiles'][0, 0].tolist()
 
 
-def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=False, q=None, ctx=None):
+def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=False, q=None, of='samples', ctx=None):
     """n_mc realisations of `res` -- jitter_run's (error='jitter') or resample_run's (error='resample') -- with the
-    posterior summaries of each over res['samples'].  Returns the dict of jitter_realisations / resample_realisations
+    posterior summaries of each over res[of]: the sample positions (of='samples') or the blobs the run saved
+    (of='blob', NestedSampler(..., blob=True)), whose summaries are the error bars of derived quantities.  Returns the dict of jitter_realisations / resample_realisations
     (logz, logzerr, h, kld; n_mc values each) plus mean (n_mc x ndim), cov (n_mc x ndim x ndim) and, with q,
     quantiles (n_mc x ndim x nq): mean_and_cov / quantile of each realisation's samples and weights
     exp(logwt - logz[-1]), a resampled point's copies counted each.  Realisation r is the stream (seed, chain0 + r):
     the one jitter_run(res, seed, chain0 + r) / resample_run(res, seed, chain0 + r) returns."""
     if error not in ('jitter', 'resample'):
         raise ValueError("Input `'error'` option '{}' is not valid.".format(error))
+    if of not in ('samples', 'blob'):
+        raise ValueError("of must be 'samples' or 'blob', not %r" % (of,))
     logl = np.asarray(res['logl'], dtype=float)
-    x = np.asarray(res['samples']) if 'samples' in res else np.empty((0, 0))
+    x = np.asarray(res[of]) if of in res else np.empty((0, 0))
     if x.ndim != 2 or len(x) != len(logl) or x.shape[1] < 1:
+        if of == 'blob':
+            raise ValueError("posterior_realisations(of='blob') needs the blob of every point (res['blob']): run the "
+                             "sampler with blob=True")
         raise ValueError("posterior_realisations needs the sample positions of every point (res['samples']); "
                          "a run made with keep_samples=False has none")
     logz_ref = _logz_end(res)
@@ -389,8 +395,8 @@ def merge_runs(res_list, ctx=None):
     into a run with the sum of their live points.  Base runs (started from the prior) merge as a pairwise tree,
     add-on runs (a dynamic batch's strands, as unravel_run makes them) merge onto the result one at a time; the
     order, the live counts, ln X (with the reference's plateau rule for equal logl) and the integrals are computed by
-    ``b2n_merge_runs``.  Positions (samples_u / samples), ncall_per_it and samples_scale are gathered here, and only
-    when every run carries them (a run made with keep_samples=False: empty positions); ncall is the sum.
+    ``b2n_merge_runs``.  Positions (samples_u / samples), ncall_per_it, samples_scale and blob are gathered here, and
+    only when every run carries them (a run made with keep_samples=False: empty positions); ncall is the sum.
 
     Deliberate differences from the reference:
       * samples_id is offset per run, so that the strands of different runs stay distinct (the reference keeps
@@ -434,7 +440,7 @@ def merge_runs(res_list, ctx=None):
     def complete(k):
         return all(k in r and len(r[k]) == len(r['logl']) for r in runs)
 
-    for k in ('ncall_per_it', 'samples_scale'):
+    for k in ('ncall_per_it', 'samples_scale', 'blob'):
         if complete(k):
             new[k] = gather(k)
     if ndims:

@@ -226,6 +226,34 @@ int b2n_model_create_user_ex(b2n_ctx* ctx, const b2n_model_desc* desc, const dou
                              const void* image, size_t image_bytes, const char* const* lowered_names,
                              int32_t* model_id);
 
+/* ---- user blobs: derived quantities of a user model, saved with every sample ------------------------------------
+ * The user's source may define a third warp-cooperative device function,
+ *
+ *     __device__ void b2n_user_blob(const double* v, double* work, int n, const double* p, int lane,
+ *                                   double* blob, int nblob);
+ *
+ *   - all 32 lanes of a warp call it; v (n doubles, read only), work (n doubles of scratch), p (the likelihood's
+ *     params, the pointer b2n_user_loglike gets) and lane are those of b2n_user_loglike, which it may call;
+ *   - blob: nblob doubles of warp-private shared memory, NaN on entry; the kernel writes them to the point's output
+ *     row after the call, so an element left unwritten is NaN;
+ *   - the caller issues __syncwarp() before and after the call; inside it, the rule of b2n_user_prior applies;
+ *   - it must be deterministic: the same v gives the same bits of the blob.
+ * The chain kernels never call it.  A blob is a function of the physical point v, so the blob of a saved sample is
+ * computed after the run by one b2n_model_blob over the samples, and equals what a chain carrying the blob of its
+ * last accepted point would hold.
+ *
+ * The program is then  #define B2N_USER_BLOB  (beside B2N_USER_PRIOR when there is a user prior), #include
+ * "b2n_user_kernels.cuh", the user's code (same options and name expressions as above).  B2N_USER_BLOB declares
+ * b2n_user_blob and adds the kernel extern "C" b2n_user_blob_kernel, which is not a slot of b2n_user_kernel_exprs:
+ * b2n_model_create_user(_ex) look it up by that name, and a model whose image lacks it has no blob.
+ *
+ * b2n_model_blob: blob (M x nblob) of the points v (M x ndim), both row-major, host or device pointers by the
+ *     pointer mode.  One warp per point.  B2N_ERR_ARG (message in b2n_last_error) for a registry model, a user model
+ *     whose image has no b2n_user_blob_kernel, nblob < 1, M < 0, or (2 ndim + nblob) doubles of staging per point
+ *     above the device's opt-in shared memory per block.  M = 0: B2N_OK, no launch.  With b2n_set_timing the call's
+ *     kernel time is b2n_last_kernel_ms. */
+int b2n_model_blob(b2n_ctx* ctx, int32_t model_id, const double* v, int64_t M, int32_t nblob, double* blob);
+
 /* ---- ellipsoid membership: MultiEllipsoid.within/overlap/contains
  *      (bounding.py:502-523), Ellipsoid.distance_many/contains (:286-305) ----
  * d2[m,k] = (x_m - c_k)^T A_k (x_m - c_k); mask[m,k] = d2 < 1 (strict != 0) or
