@@ -165,12 +165,13 @@ def merge_two(saved, new, logl_min):
     return out
 
 
-def integrate_record(rec):
-    """ln X from the live counts (combine_runs :1560-1585, no plateau mode: continuous likelihoods), then the
+def integrate_record(rec, logvol_init=0.0):
+    """ln X from the live counts (combine_runs :1560-1585, no plateau mode: continuous likelihoods), starting at
+    `logvol_init`, the ln X of the base run's initial live points (``NestedSampler.initial_logvol``), then the
     trapezoid integrals (utils.compute_integrals)."""
     n = rec['n'].astype(float)
-    logvol = -np.cumsum(np.log((n + 1.) / n))
-    logwt, logz, logzvar, h = _integrate(rec['logl'], logvol)
+    logvol = logvol_init - np.cumsum(np.log((n + 1.) / n))
+    logwt, logz, logzvar, h = _integrate(rec['logl'], logvol, logvol_init=logvol_init)
     return logvol, logwt, logz, logzvar, h
 
 
@@ -187,6 +188,7 @@ class DynamicNestedSampler:
         self.ncall = 0
         self.batch_bounds = []
         self.results = None
+        self.logvol_init = 0.0            # ln X of the baseline's initial live points (sample_initial)
         self.strands = False              # record samples_id / samples_it (run_nested(strands=True))
 
     def _sampler(self, nlive, seed, live_points=None):
@@ -208,7 +210,7 @@ class DynamicNestedSampler:
 
     def _results(self):
         rec = self.saved
-        logvol, logwt, logz, logzvar, h = integrate_record(rec)
+        logvol, logwt, logz, logzvar, h = integrate_record(rec, self.logvol_init)
         self.results = Results(niter=len(rec['logl']), ncall=int(self.ncall), eff=100. * len(rec['logl']) / max(self.ncall, 1),
                                samples_u=rec['u'], samples=rec['v'], logl=rec['logl'], logvol=logvol, logwt=logwt, logz=logz,
                                logzerr=np.sqrt(logzvar), information=h, samples_n=rec['n'], samples_scale=rec['scale'],
@@ -228,6 +230,7 @@ class DynamicNestedSampler:
         self.saved = self._record(res, 0)
         self.ncall = int(res['ncall'])
         self.base_sampler = s
+        self.logvol_init = s.logvol_init
         self.batch_bounds = [(-np.inf, np.inf)]
         return self._results()
 
@@ -293,7 +296,7 @@ class DynamicNestedSampler:
                 bs.live_it = np.zeros(nlive, dtype=np.int64)     # the batch's points start its strands
             # join the saved run where it crosses logl_min (:598-606): ln X and ln Z there start the batch's dlogz test
             vol_idx = 0 if not np.isfinite(logl_min) else int(np.argmin(np.abs(saved_logl - logl_min))) + 1
-            lv0 = float(saved_logvol[vol_idx - 1]) if vol_idx > 0 else 0.0
+            lv0 = float(saved_logvol[vol_idx - 1]) if vol_idx > 0 else self.logvol_init
             lz0 = float(res['logz'][vol_idx - 1]) if vol_idx > 0 else nested.LOWL
             dev = bs._device_rounds(lz0, lv0, logl_min if np.isfinite(logl_min) else nested.LOWL, dlogz,
                                     maxiter if maxiter is not None else 1 << 62, maxcall, round_size,

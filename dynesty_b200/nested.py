@@ -57,12 +57,14 @@ class Results(dict):
         return mean, (d * w[:, None]).T @ d
 
 
-def _integrate(logl, logvol, reweight=None):
+def _integrate(logl, logvol, reweight=None, logvol_init=0.0):
     """Trapezoid evidence / information integrals over the dead-point sequence
     (utils.py:1411-1467 compute_integrals, same quadrature); reweight: the log-reweight added to every logwt, as
-    compute_integrals(reweight=) does (h keeps the unreweighted likelihoods, normalised by the reweighted logz[-1])."""
+    compute_integrals(reweight=) does (h keeps the unreweighted likelihoods, normalised by the reweighted logz[-1]).
+    logvol_init: ln X where the sequence starts (``NestedSampler.initial_logvol``); the first interval is
+    [X_1, X_init], not [X_1, 1], so the prior volume where logl is -inf carries no weight."""
     lpad = np.concatenate([[LOWL], logl])
-    dlv = np.diff(logvol, prepend=0)
+    dlv = np.diff(logvol, prepend=logvol_init)
     logdvol = logvol - dlv + np.log1p(-np.exp(dlv))
     logdvol2 = logdvol + math.log(0.5)
     logwt = np.logaddexp(lpad[1:], lpad[:-1]) + logdvol2
@@ -177,6 +179,12 @@ class NestedSampler:
         # -- live points (sampler.py:56-262, evaluated in one launch)
         if live_points is not None:         # (u, v, logl[, blobs]) supplied by the caller (dynesty.py:600 `live_points`)
             self.live_u, self.live_v, self.live_logl = (np.array(a, dtype=float) for a in live_points[:3])
+            bad = np.nonzero(~np.isfinite(self.live_logl))[0]
+            if len(bad):
+                # the reference's -inf -> LOWL route needs plateau mode (ties in the live set), which this code lacks
+                raise ValueError('live point %d has a non-finite log-likelihood (%r): every supplied live point needs '
+                                 'a finite logl' % (bad[0], self.live_logl[bad[0]]))
+            ndraws = self.nlive
         elif live_init == 'device':
             # _initialize_live_points (sampler.py:56-262) on the device: nlive prior draws + transform + likelihood in
             # ONE launch (b2n_unitcube_batch at threshold -inf: a draw whose logl is -inf is redrawn, the reference's
@@ -184,12 +192,13 @@ class NestedSampler:
             from . import ops
             o = ops.unitcube_batch(model.model_id(ctx), self.nlive, n, -np.inf, self.seed, chain0=1 << 61, ctx=ctx)
             self.live_u, self.live_v, self.live_logl = o['u'], o['v'], o['logl']
-            self.init_ncall = int(o['ncall'].sum())
+            ndraws = int(o['ncall'].sum())
         else:
-            self.live_u = self.rstate.random((self.nlive, n))
-            self.live_v, self.live_logl = model.evaluate(self.live_u, ctx=ctx)
+            ndraws = self._host_init(model, ctx)
+        self.logvol_init = self.initial_logvol(self.nlive, ndraws)
+        self.init_ncall = ndraws
         self.it = 1
-        self.ncall = getattr(self, 'init_ncall', self.nlive)
+        self.ncall = ndraws
         self.eff = 0.
         self.nbound = 1
         self.chain_counter = 0
@@ -201,6 +210,41 @@ class NestedSampler:
         self._qpos = 0
         self.live_it = None               # strands recorded (run_nested(strands=True)): per slot, the dead points
                                           # of the run recorded before its occupant entered the live set
+
+    @staticmethod
+    def initial_logvol(nlive, ndraws):
+        """ln X at the start of the run: the live points are uniform over the region where logl is finite, and
+        rejection sampling estimates its prior volume as f = nlive / ndraws, the number of finite points kept over
+        the number of prior draws spent to find them.  Exactly 0.0 when every draw was kept.  (The reference instead
+        fills the live set up with LOWL points and starts at -ln(attempts), which relies on its plateau mode.)"""
+        return 0.0 if ndraws == nlive else math.log(nlive / ndraws)
+
+    def _host_init(self, model, ctx):
+        """The reference's rejection loop (sampler.py:113-219): batches of nlive prior draws from `rstate`, the finite
+        points taken in order.  Returns the number of draws up to the last point taken.  NaN or +inf logl is an
+        error; no finite point in 1000 batches is an error."""
+        N, n = self.nlive, self.ndim
+        us, vs, ls = [], [], []
+        have, ndraws = 0, 0
+        for attempt in range(1, 1 << 62):
+            u = self.rstate.random((N, n))
+            v, logl = model.evaluate(u, ctx=ctx)
+            if np.any(np.isnan(logl) | (logl == np.inf)):
+                raise ValueError('The log-likelihood of a live point is invalid (NaN or +inf).')
+            ok = np.nonzero(logl > -np.inf)[0][:N - have]
+            us.append(u[ok])
+            vs.append(v[ok])
+            ls.append(logl[ok])
+            have += len(ok)
+            if have == N:
+                ndraws += int(ok[-1]) + 1
+                break
+            ndraws += N
+            if have == 0 and attempt >= 1000:
+                raise RuntimeError('After %d batches of %d prior draws no point has a finite log-likelihood.'
+                                   % (attempt, N))
+        self.live_u, self.live_v, self.live_logl = np.concatenate(us), np.concatenate(vs), np.concatenate(ls)
+        return ndraws
 
     # ------------------------------------------------------------------ save / restore (utils.py:2321-2355)
     def __getstate__(self):
@@ -594,7 +638,7 @@ class NestedSampler:
         heap = [(float(l), i) for i, l in enumerate(self.live_logl)]
         heapq.heapify(heap)
         lmax = float(self.live_logl.max())
-        logz, logvol, loglstar = LOWL, 0.0, LOWL
+        logz, logvol, loglstar = LOWL, self.logvol_init, LOWL
         cap = 4 * nlive
         dead_u = np.empty((cap, self.ndim))
         dead_v = np.empty((cap, self.ndim))
@@ -667,7 +711,7 @@ class NestedSampler:
             self.it += 1
         # ---- results (+ remaining live points, sampler.py:780-914)
         logl = dead_l[:ndead]
-        logvols = -dlv * np.arange(1, ndead + 1)
+        logvols = self.logvol_init - dlv * np.arange(1, ndead + 1)
         su, sv, nc_all = dead_u[:ndead], dead_v[:ndead], dead_nc[:ndead]
         host_str = (dead_id[:ndead].copy(), dead_it[:ndead].copy()) if strands else None
         if hand_over:
@@ -712,7 +756,7 @@ class NestedSampler:
             ndead = len(logl)
         if add_live:
             order = np.argsort(self.live_logl)
-            lv_live = np.log(1. - (np.arange(nlive) + 1.) / (nlive + 1.)) + (logvols[-1] if ndead else 0.0)
+            lv_live = np.log(1. - (np.arange(nlive) + 1.) / (nlive + 1.)) + (logvols[-1] if ndead else self.logvol_init)
             logl = np.concatenate([logl, self.live_logl[order]])
             logvols = np.concatenate([logvols, lv_live])
             if have_pos:
@@ -731,7 +775,7 @@ class NestedSampler:
         cum = np.cumsum(nc_all)
         sample_scale = (sh[np.minimum(np.searchsorted(sh[:, 0], cum + (self.nlive if len(cum) else 0)), len(sh) - 1), 1]
                         if len(sh) else np.ones(len(nc_all)))
-        logwt, logzs, logzvar, h = _integrate(logl, logvols)
+        logwt, logzs, logzvar, h = _integrate(logl, logvols, logvol_init=self.logvol_init)
         self.results = Results(niter=ndead, ncall=int(self.ncall), eff=100. * ndead / max(self.ncall, 1),
                                samples_u=su, samples=sv, logl=logl, logvol=logvols, logwt=logwt, logz=logzs,
                                logzerr=np.sqrt(logzvar), information=h, ncall_per_it=nc_all,
