@@ -362,10 +362,10 @@ static __device__ __forceinline__ bool sweep_inverse_regs(const double* __restri
 // break-down, condition bound, slow power iteration: near-degenerate leading eigenvalues) is flagged
 // `suspect` and the caller redoes the whole update with the eigen path.  Accepted leaves are always
 // re-fitted with the eigen path (they need axes / axlens), so outputs never come from this kernel.
-// PART 0: the whole candidate fit in one launch.  The fit is two INDEPENDENT latency chains that both start from the
-// raw covariance -- (1) Cholesky -> L^-1 -> am, pivots, conditioning; (2) repeated squaring -> major axis -- so the
-// caller may run them as two launches on two streams (PART 1 on the main stream, PART 2 on a side stream; they
-// write disjoint outputs and disjoint words of the node's NodeStat: `suspect` / `pad`), b2n_process_nodes.
+// The fit is two INDEPENDENT latency chains that both start from the raw covariance -- (1) Cholesky -> L^-1 -> am,
+// pivots, conditioning; (2) repeated squaring -> major axis -- run as two launches on two streams (PART 1 on the main
+// stream, PART 2 on a side stream; they write disjoint outputs and disjoint words of the node's NodeStat:
+// `suspect` / `pad`), b2n_fit_candidates.
 template <int PART>
 __global__ void __launch_bounds__(512) chol_node_kernel(NodeArrays na, const int* __restrict__ nodelist) {
     extern __shared__ double sm[];
@@ -385,28 +385,23 @@ __global__ void __launch_bounds__(512) chol_node_kernel(NodeArrays na, const int
     double* Cm = na.cov + (size_t)node * nn;
     NodeStat* st = na.stat + node;
     if (tid == 0) { s_bad = 0; s_it = 0; }
-    double cnorm = 0.0, anorm = 0.0;
-    if (PART != 2) {
+    if (PART == 1) {
     // ---- precision matrix, pivots, |cov|_inf |am|_inf: symmetric sweeps on a register-resident matrix
     //      (sweep_inverse_regs above)
+    double cnorm = 0.0, anorm = 0.0;
     double* AM = na.am + (size_t)node * nn;
     __syncthreads();
     const bool okA = (n <= 64) ? sweep_inverse_regs<4, 2>(src, Cm, AM, n, ybuf, dg, red, &s_bad, cnorm, anorm)
                                : sweep_inverse_regs<8, 4>(src, Cm, AM, n, ybuf, dg, red, &s_bad, cnorm, anorm);
     if (!okA) {
-        if (tid == 0) {
-            st->suspect = 1; st->good = 1; st->fallback = 0; st->retry = 0;
-            if (PART == 0) { st->sweeps = 0; st->pad = 0; }
-        }
+        if (tid == 0) { st->suspect = 1; st->good = 1; st->fallback = 0; st->retry = 0; }
         for (int k = tid; k < n; k += T) na.lam[(size_t)node * n + k] = 1.0;
         return;
     }
     for (int k = tid; k < n; k += T) na.lam[(size_t)node * n + k] = dg[k];
-    if (PART == 1) {
-        if (tid == 0) { st->suspect = (cnorm * anorm < 1e10) ? 0 : 1; st->good = 1; st->fallback = 0; st->retry = 0; }
-        return;
-    }
-    }   // PART != 2
+    if (tid == 0) { st->suspect = (cnorm * anorm < 1e10) ? 0 : 1; st->good = 1; st->fallback = 0; st->retry = 0; }
+    return;
+    }   // PART == 1
     __syncthreads();
     // ---- major axis.  Plain power iteration stalls on the deep nodes of the tree (a half of a half of a
     //      Gaussian cloud has a leading eigenvalue within a few % of the next ones), so the dominant
@@ -538,19 +533,9 @@ __global__ void __launch_bounds__(512) chol_node_kernel(NodeArrays na, const int
         const int i = (int)(e / n), j = (int)(e - (size_t)i * n);
         AX[e] = (j == n - 1) ? sgn * v[i] * ax : 0.0;
     }
-    if (tid == 0) {
-        if (PART == 2) {            // the major-axis half reports through its own word
-            st->pad = (conv && lam > 0.0) ? 0 : 1;
-            st->sweeps = it;
-        } else {
-            const bool ok = conv && (cnorm * anorm < 1e10) && (lam > 0.0);
-            st->suspect = ok ? 0 : 1;
-            st->good = 1;
-            st->fallback = 0;
-            st->sweeps = it;
-            st->retry = 0;
-            st->pad = 0;
-        }
+    if (tid == 0) {                 // the major-axis half reports through its own word
+        st->pad = (conv && lam > 0.0) ? 0 : 1;
+        st->sweeps = it;
     }
 }
 
@@ -689,199 +674,205 @@ int b2n_boundwork_init(b2n_ctx* ctx, BoundWork& w, const double* dP, int64_t N, 
     return B2N_OK;
 }
 
-// Full bounding_ellipsoid (bounding.py:1387-1461) for every node in `refs`.
-// On return `stats` holds the per-node NodeStat (host copy); the stream is synchronised.
-int b2n_process_nodes(BoundWork& w, const std::vector<NodeRef>& refs_in, std::vector<NodeStat>& stats,
-                      bool candidate, bool defer) {
-    b2n_ctx* ctx = w.ctx;
-    const int n = w.n;
-    const size_t nn = (size_t)n * n;
-    std::vector<NodeRef> refs = refs_in;
+// the jobs of a batch of nodes (b2n_rows_per_job rows each, slots numbered from 0); sets each ref's slot0 / nslots
+static std::vector<JobL> node_jobs(std::vector<NodeRef>& refs, int64_t N) {
+    const int rows = b2n_rows_per_job(N);
     std::vector<JobL> jobs;
-    int slot = 0;
-    for (auto& r : refs) {
-        r.slot0 = slot;
-        for (int a = r.start; a < r.start + r.count; a += b2n_rows_per_job(w.N)) {
-            JobL j;
-            memset(&j, 0, sizeof(j));
-            j.node = r.node; j.r0 = a; j.r1 = std::min(a + b2n_rows_per_job(w.N), r.start + r.count);
-            j.slot = slot++; j.level = r.level;
-            jobs.push_back(j);
-        }
-        r.nslots = slot - r.slot0;
+    for (NodeRef& r : refs) {
+        r.slot0 = (int)jobs.size();
+        for (int a = r.start; a < r.start + r.count; a += rows)
+            jobs.push_back(JobL{r.node, a, std::min(a + rows, r.start + r.count), (int)jobs.size(), r.level, 0, 0, 0});
+        r.nslots = (int)jobs.size() - r.slot0;
     }
-    const int nnodes = (int)refs.size(), njobs = (int)jobs.size();
-    if (nnodes == 0) return B2N_OK;
-    std::vector<int> nodelist(nnodes);
-    for (int i = 0; i < nnodes; i++) nodelist[i] = refs[i].node;
+    return jobs;
+}
 
+// a batch of nodes on the device: its jobs (ctx->scratch4), refs (scratch5) and node ids (work0)
+struct NodeBatch {
+    int nnodes, njobs;
+    const JobL* jobs;
+    const NodeRef* refs;
+    const int* list;
+};
+
+static int stage_nodes(BoundWork& w, std::vector<NodeRef> refs, NodeBatch& b) {
+    b2n_ctx* ctx = w.ctx;
+    const std::vector<JobL> jobs = node_jobs(refs, w.N);
+    std::vector<int> list;
+    for (const NodeRef& r : refs) list.push_back(r.node);
     const void *djobs, *drefs, *dlist;
     B2N_TRY(b2n_in_host(ctx, ctx->scratch4, jobs.data(), jobs.size() * sizeof(JobL), &djobs));
     B2N_TRY(b2n_in_host(ctx, ctx->scratch5, refs.data(), refs.size() * sizeof(NodeRef), &drefs));
-    B2N_TRY(b2n_in_host(ctx, ctx->work0, nodelist.data(), nodelist.size() * sizeof(int), &dlist));
-    B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)njobs * std::max(nn, (size_t)n) * sizeof(double)));
+    B2N_TRY(b2n_in_host(ctx, ctx->work0, list.data(), list.size() * sizeof(int), &dlist));
+    b = NodeBatch{(int)refs.size(), (int)jobs.size(), (const JobL*)djobs, (const NodeRef*)drefs, (const int*)dlist};
+    return B2N_OK;
+}
+
+// mean and sample covariance of every node of the batch -> na.mean / na.covraw; the per-job partials go to
+// ctx->scratch1, which the fmax scan reuses
+static int launch_moments(BoundWork& w, const NodeBatch& b) {
+    b2n_ctx* ctx = w.ctx;
+    const int n = w.n;
+    const size_t nn = (size_t)n * n;
+    B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)b.njobs * std::max(nn, (size_t)n) * sizeof(double)));
     double* partial = ctx->scratch1.as<double>();
     cudaStream_t st = ctx->stream;
-
-    // moments
-    colsum_partial_kernel<<<njobs, 256, (size_t)8 * n * sizeof(double), st>>>(w.P, w.perm, w.N, n, (const JobL*)djobs, partial);
+    colsum_partial_kernel<<<b.njobs, 256, (size_t)8 * n * sizeof(double), st>>>(w.P, w.perm, w.N, n, b.jobs, partial);
     B2N_LAUNCH_CHECK(ctx);
-    mean_finalize_kernel<<<nnodes, 128, 0, st>>>((const NodeRef*)drefs, n, partial, w.na.mean);
+    mean_finalize_kernel<<<b.nnodes, 128, 0, st>>>(b.refs, n, partial, w.na.mean);
     B2N_LAUNCH_CHECK(ctx);
     const int ntile = (n + B2N_TILE - 1) / B2N_TILE;
-    cov_partial_kernel<<<dim3(njobs, ntile * (ntile + 1) / 2), 256, 0, st>>>(w.P, w.perm, w.N, n, (const JobL*)djobs,
-                                                                            w.na.mean, partial, ntile);
+    cov_partial_kernel<<<dim3(b.njobs, ntile * (ntile + 1) / 2), 256, 0, st>>>(w.P, w.perm, w.N, n, b.jobs, w.na.mean,
+                                                                              partial, ntile);
     B2N_LAUNCH_CHECK(ctx);
-    cov_finalize_kernel<<<dim3(nnodes, (unsigned)std::min<size_t>((nn + 255) / 256, 64)), 256, 0, st>>>(
-        (const NodeRef*)drefs, n, partial, w.na.covraw);
+    cov_finalize_kernel<<<dim3(b.nnodes, (unsigned)std::min<size_t>((nn + 255) / 256, 64)), 256, 0, st>>>(
+        b.refs, n, partial, w.na.covraw);
     B2N_LAUNCH_CHECK(ctx);
+    return B2N_OK;
+}
 
-    // eigen + ladder
-    const int ld = w.na.ld, half = ((n + 1) & ~1) / 2;
+// fmax scan of the batch's rows, then rescale + volume of its nodes; `wait`: an event the finish waits for
+static int launch_fmax_finish(BoundWork& w, const NodeBatch& b, int pass, cudaEvent_t wait = nullptr) {
+    b2n_ctx* ctx = w.ctx;
+    cudaStream_t st = ctx->stream;
+    double* partial = ctx->scratch1.as<double>();
+    fmax_partial_kernel<<<dim3(b.njobs, B2N_FMAX_SUB), 256, (size_t)8 * w.n * sizeof(double), st>>>(w.P, w.perm, w.N,
+                                                                                                  w.na, b.jobs, partial);
+    B2N_LAUNCH_CHECK(ctx);
+    if (wait) B2N_CUDA(ctx, cudaStreamWaitEvent(st, wait, 0));
+    scale_finish_kernel<<<b.nnodes, 1024, 0, st>>>(w.na, b.refs, partial, pass, w.logvol_pref, B2N_FMAX_SUB);
+    B2N_LAUNCH_CHECK(ctx);
+    return B2N_OK;
+}
+
+// The single-CTA eigen solve (eig_ladder_kernel): both n x ld work matrices in shared memory when they fit, else in a
+// global workspace of gwork_bytes per node (used only if the sliced solver cannot take the matrix either).  One
+// HALF-warp per rotation pair of a Jacobi round (n/2 pairs), at least 4 warps for the O(n^2) loops.
+struct EigPlan {
+    bool smem;
+    size_t smem_bytes, gwork_bytes;
+    int threads;
+};
+
+static EigPlan eig_plan(const BoundWork& w) {
+    const int n = w.n, half = ((n + 1) & ~1) / 2;
     const size_t small_b = (size_t)(2 * half + 2 * n + 32) * sizeof(double);
-    const size_t mats_b = (size_t)2 * n * ld * sizeof(double);
-    const int use_smem = small_b + mats_b <= (size_t)ctx->max_smem_optin ? 1 : 0;
-    const size_t eig_smem = small_b + (use_smem ? mats_b : 0);
+    const size_t mats_b = (size_t)2 * n * w.na.ld * sizeof(double);
+    const bool smem = small_b + mats_b <= (size_t)w.ctx->max_smem_optin;
+    return EigPlan{smem, small_b + (smem ? mats_b : 0), mats_b, 32 * std::max(4, std::min(32, (half + 1) / 2))};
+}
+
+static int launch_eig(BoundWork& w, const EigPlan& p, const NodeArrays& na, const int* dlist, int pn, int pass,
+                      double* gwork, cudaStream_t st) {
+    b2n_ctx* ctx = w.ctx;
+    if (p.smem) {
+        B2N_TRY(b2n_func_smem(ctx, (const void*)(eig_ladder_kernel<true>), p.smem_bytes));
+        eig_ladder_kernel<true><<<pn, p.threads, p.smem_bytes, st>>>(na, dlist, pass, gwork);
+    } else {
+        B2N_TRY(b2n_func_smem(ctx, (const void*)(eig_ladder_kernel<false>), p.smem_bytes));
+        eig_ladder_kernel<false><<<pn, p.threads, p.smem_bytes, st>>>(na, dlist, pass, gwork);
+    }
+    B2N_LAUNCH_CHECK(ctx);
+    return B2N_OK;
+}
+
+// a high-priority non-blocking stream and its two events, created on first use
+static int side_stream(b2n_ctx* ctx, cudaStream_t& s, cudaEvent_t& done, cudaEvent_t& go) {
+    if (s) return B2N_OK;
+    int lo = 0, hi = 0;
+    if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess) { cudaGetLastError(); hi = 0; }
+    B2N_CUDA(ctx, cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, hi));
+    B2N_CUDA(ctx, cudaEventCreateWithFlags(&done, cudaEventDisableTiming));
+    B2N_CUDA(ctx, cudaEventCreateWithFlags(&go, cudaEventDisableTiming));
+    return B2N_OK;
+}
+
+// Full bounding_ellipsoid (bounding.py:1387-1461) for every node in `refs`.
+// On return `stats` holds the per-node NodeStat (host copy); the stream is synchronised.
+int b2n_fit_nodes(BoundWork& w, const std::vector<NodeRef>& refs, std::vector<NodeStat>& stats) {
+    b2n_ctx* ctx = w.ctx;
+    const int nnodes = (int)refs.size();
+    if (nnodes == 0) return B2N_OK;
+    cudaStream_t st = ctx->stream;
+    NodeBatch b;
+    B2N_TRY(stage_nodes(w, refs, b));
+    B2N_TRY(launch_moments(w, b));
+    // eigen + ladder.  large n: packed-triangle / column-sliced Jacobi (b2n_eig_sliced.cu); else the single-CTA kernel
+    const EigPlan ep = eig_plan(w);
     double* gwork = nullptr;
-    if (!use_smem) {       // only used if the sliced path cannot take the matrix either
-        B2N_CUDA(ctx, ctx->scratch2.ensure((size_t)nnodes * mats_b));
+    if (!ep.smem) {
+        B2N_CUDA(ctx, ctx->scratch2.ensure((size_t)nnodes * ep.gwork_bytes));
         gwork = ctx->scratch2.as<double>();
     }
-    B2N_TRY(b2n_func_smem(ctx, use_smem ? (const void*)(eig_ladder_kernel<true>) : (const void*)(eig_ladder_kernel<false>), (size_t)(eig_smem)));
-    // one HALF-warp per rotation pair of a Jacobi round (n/2 pairs), at least 4 warps for the O(n^2) loops
-    const int eig_threads = 32 * std::max(4, std::min(32, (half + 1) / 2));
-    const size_t fm_smem = (size_t)8 * n * sizeof(double);
-
-    std::vector<NodeStat> hs(nnodes);
+    std::vector<NodeStat> hs(nnodes), all;
+    std::vector<int> which(nnodes);
+    for (int i = 0; i < nnodes; i++) which[i] = i;
     for (int pass = 0; pass < 2; pass++) {
-        const void* plist = dlist;
-        const void* prefs = drefs;
-        const void* pjobs = djobs;
-        int pn = nnodes, pj = njobs;
-        std::vector<NodeRef> refs2;
-        std::vector<JobL> jobs2;
-        std::vector<int> list2;
         if (pass == 1) {
             // second pass only for nodes whose matrix needed repair (:1454-1457)
-            int s2 = 0;
-            for (int i = 0; i < nnodes; i++) {
-                if (hs[i].good || hs[i].error) continue;
-                NodeRef r = refs[i];
-                r.slot0 = s2;
-                for (int a = r.start; a < r.start + r.count; a += b2n_rows_per_job(w.N)) {
-                    JobL j;
-                    memset(&j, 0, sizeof(j));
-                    j.node = r.node; j.r0 = a; j.r1 = std::min(a + b2n_rows_per_job(w.N), r.start + r.count);
-                    j.slot = s2++; j.level = r.level;
-                    jobs2.push_back(j);
-                }
-                r.nslots = s2 - r.slot0;
-                refs2.push_back(r);
-                list2.push_back(r.node);
-            }
+            std::vector<NodeRef> refs2;
+            which.clear();
+            for (int i = 0; i < nnodes; i++)
+                if (!hs[i].good && !hs[i].error) { refs2.push_back(refs[i]); which.push_back(i); }
             if (refs2.empty()) break;
-            B2N_TRY(b2n_in_host(ctx, ctx->scratch4, jobs2.data(), jobs2.size() * sizeof(JobL), &pjobs));
-            B2N_TRY(b2n_in_host(ctx, ctx->scratch5, refs2.data(), refs2.size() * sizeof(NodeRef), &prefs));
-            B2N_TRY(b2n_in_host(ctx, ctx->work0, list2.data(), list2.size() * sizeof(int), &plist));
-            pn = (int)refs2.size();
-            pj = (int)jobs2.size();
+            B2N_TRY(stage_nodes(w, refs2, b));
         }
-        // large n: packed-triangle / column-sliced Jacobi (b2n_eig_sliced.cu); else the single-CTA kernel
         int sliced = 0;
-        bool chol_split = false;
-        if (candidate) {            // Cholesky path (pass 0 only: certified nodes never need the second pass)
-            const size_t csm = (size_t)(2 * n * ld + 3 * n + 32 + 2 * (n + 2)) * sizeof(double);
-            const char* cenv = getenv("B2N_CHOL_SPLIT");
-            chol_split = !(cenv && cenv[0] == '0');
-            if (chol_split && !ctx->stream_side2) {
-                int lo = 0, hi = 0;
-                if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess) { cudaGetLastError(); hi = 0; }
-                B2N_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->stream_side2, cudaStreamNonBlocking, hi));
-                B2N_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_side2, cudaEventDisableTiming));
-                B2N_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_side2_go, cudaEventDisableTiming));
-            }
-            if (chol_split) {
-                // the two halves of the candidate fit side by side: the major axes (repeated squaring) on the side
-                // stream, Cholesky / precision matrix / fmax scan on the main one; they meet before scale_finish
-                // (which rescales the axes)
-                B2N_TRY(b2n_func_smem(ctx, (const void*)(chol_node_kernel<1>), (size_t)(csm)));
-                B2N_TRY(b2n_func_smem(ctx, (const void*)(chol_node_kernel<2>), (size_t)(csm)));
-                B2N_CUDA(ctx, cudaEventRecord(ctx->ev_side2_go, st));
-                B2N_CUDA(ctx, cudaStreamWaitEvent(ctx->stream_side2, ctx->ev_side2_go, 0));
-                chol_node_kernel<2><<<pn, 512, csm, ctx->stream_side2>>>(w.na, (const int*)plist);
-                B2N_LAUNCH_CHECK(ctx);
-                B2N_CUDA(ctx, cudaEventRecord(ctx->ev_side2, ctx->stream_side2));
-                chol_node_kernel<1><<<pn, 512, csm, st>>>(w.na, (const int*)plist);
-                B2N_LAUNCH_CHECK(ctx);
-            } else {
-                B2N_TRY(b2n_func_smem(ctx, (const void*)(chol_node_kernel<0>), (size_t)(csm)));
-                chol_node_kernel<0><<<pn, 512, csm, st>>>(w.na, (const int*)plist);
-                B2N_LAUNCH_CHECK(ctx);
-            }
-        } else if (!use_smem) B2N_TRY(b2n_eig_sliced(w, (const int*)plist, pn, pass, 0, &sliced));
-        if (!candidate && !sliced) {
-            if (use_smem) eig_ladder_kernel<true><<<pn, eig_threads, eig_smem, st>>>(w.na, (const int*)plist, pass, gwork);
-            else eig_ladder_kernel<false><<<pn, eig_threads, eig_smem, st>>>(w.na, (const int*)plist, pass, gwork);
-            B2N_LAUNCH_CHECK(ctx);
-        }
-        fmax_partial_kernel<<<dim3(pj, B2N_FMAX_SUB), 256, fm_smem, st>>>(w.P, w.perm, w.N, w.na, (const JobL*)pjobs, partial);
-        B2N_LAUNCH_CHECK(ctx);
-        if (chol_split) B2N_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_side2, 0));
-        scale_finish_kernel<<<pn, 1024, 0, st>>>(w.na, (const NodeRef*)prefs, partial, pass, w.logvol_pref, B2N_FMAX_SUB);
-        B2N_LAUNCH_CHECK(ctx);
-        // candidates of a tree being expanded: nothing on the host depends on their stats before the end of the
-        // expansion (a certified candidate never takes the second pass) -- the caller reads them all at once
-        // (b2n_read_stats) and the next level's launches queue behind these without a host round trip
-        if (candidate && defer) return B2N_OK;
-        // read back the node stats (one copy of the whole small array)
+        if (!ep.smem) B2N_TRY(b2n_eig_sliced(w, b.list, b.nnodes, pass, 0, &sliced));
+        if (!sliced) B2N_TRY(launch_eig(w, ep, w.na, b.list, b.nnodes, pass, gwork, st));
+        B2N_TRY(launch_fmax_finish(w, b, pass));
         B2N_CUDA(ctx, cudaStreamSynchronize(st));
-        std::vector<NodeStat> all(w.cap);
-        B2N_CUDA(ctx, b2n_copy_sync(ctx, all.data(), w.na.stat, (size_t)w.cap * sizeof(NodeStat), cudaMemcpyDeviceToHost));
-        for (int i = 0; i < nnodes; i++) {
-            if (pass == 1 && (hs[i].good || hs[i].error)) continue;
-            hs[i] = all[refs[i].node];
-        }
-        // sliced path: the repair ladder is one decomposition per launch -> re-run the nodes whose
-        // covariance was modified (rare: rank-deficient / ill-conditioned clouds), up to 100 trials
+        B2N_TRY(b2n_read_stats(w, all));
+        for (int i : which) hs[i] = all[refs[i].node];
+        // sliced path: the repair ladder is one decomposition per launch -> re-run the nodes whose covariance was
+        // modified (rare: rank-deficient / ill-conditioned clouds).  Attempt 99 is a node's 100th decomposition, at
+        // which eig_check_kernel ends the ladder (identity fallback, retry cleared): no node is left to retry.
         for (int attempt = 1; sliced && attempt < 100; attempt++) {
             std::vector<NodeRef> refs3;
-            std::vector<JobL> jobs3;
-            std::vector<int> list3, which;
-            int s3 = 0;
-            for (int i = 0; i < nnodes; i++) {
-                if (!hs[i].retry) continue;
-                NodeRef r = refs[i];
-                r.slot0 = s3;
-                for (int a = r.start; a < r.start + r.count; a += b2n_rows_per_job(w.N)) {
-                    JobL j;
-                    memset(&j, 0, sizeof(j));
-                    j.node = r.node; j.r0 = a; j.r1 = std::min(a + b2n_rows_per_job(w.N), r.start + r.count);
-                    j.slot = s3++; j.level = r.level;
-                    jobs3.push_back(j);
-                }
-                r.nslots = s3 - r.slot0;
-                refs3.push_back(r);
-                list3.push_back(r.node);
-                which.push_back(i);
-            }
+            std::vector<int> again;
+            for (int i = 0; i < nnodes; i++)
+                if (hs[i].retry) { refs3.push_back(refs[i]); again.push_back(i); }
             if (refs3.empty()) break;
-            const void *j3, *r3, *l3;
-            B2N_TRY(b2n_in_host(ctx, ctx->scratch4, jobs3.data(), jobs3.size() * sizeof(JobL), &j3));
-            B2N_TRY(b2n_in_host(ctx, ctx->scratch5, refs3.data(), refs3.size() * sizeof(NodeRef), &r3));
-            B2N_TRY(b2n_in_host(ctx, ctx->work0, list3.data(), list3.size() * sizeof(int), &l3));
+            NodeBatch r;
+            B2N_TRY(stage_nodes(w, refs3, r));
             int used = 0;
-            B2N_TRY(b2n_eig_sliced(w, (const int*)l3, (int)refs3.size(), pass, 1, &used));
-            fmax_partial_kernel<<<dim3((unsigned)jobs3.size(), B2N_FMAX_SUB), 256, fm_smem, st>>>(w.P, w.perm, w.N, w.na, (const JobL*)j3, partial);
-            B2N_LAUNCH_CHECK(ctx);
-            scale_finish_kernel<<<(unsigned)refs3.size(), 1024, 0, st>>>(w.na, (const NodeRef*)r3, partial, pass, w.logvol_pref, B2N_FMAX_SUB);
-            B2N_LAUNCH_CHECK(ctx);
+            B2N_TRY(b2n_eig_sliced(w, r.list, r.nnodes, pass, 1, &used));
+            B2N_TRY(launch_fmax_finish(w, r, pass));
             B2N_CUDA(ctx, cudaStreamSynchronize(st));
-            B2N_CUDA(ctx, b2n_copy_sync(ctx, all.data(), w.na.stat, (size_t)w.cap * sizeof(NodeStat), cudaMemcpyDeviceToHost));
-            for (int i : which) hs[i] = all[refs[i].node];
+            B2N_TRY(b2n_read_stats(w, all));
+            for (int i : again) hs[i] = all[refs[i].node];
         }
     }
     stats = hs;
     return B2N_OK;
+}
+
+// The candidates of a multi-ellipsoid tree through the Cholesky path (chol_node_kernel): moments, then the two halves
+// of the fit side by side -- the major axes (repeated squaring) on a side stream, Cholesky / precision matrix / fmax
+// scan on the main one -- meeting before scale_finish (which rescales the axes).  Nothing on the host depends on a
+// candidate's stats before the end of the expansion (a certified candidate never takes the second pass): this only
+// enqueues, the caller reads them all at once (b2n_read_stats) and the next level's launches queue behind these
+// without a host round trip.
+int b2n_fit_candidates(BoundWork& w, const std::vector<NodeRef>& refs) {
+    b2n_ctx* ctx = w.ctx;
+    if (refs.empty()) return B2N_OK;
+    const int n = w.n, ld = w.na.ld;
+    cudaStream_t st = ctx->stream;
+    NodeBatch b;
+    B2N_TRY(stage_nodes(w, refs, b));
+    B2N_TRY(launch_moments(w, b));
+    B2N_TRY(side_stream(ctx, ctx->stream_side2, ctx->ev_side2, ctx->ev_side2_go));
+    const size_t csm = (size_t)(2 * n * ld + 3 * n + 32 + 2 * (n + 2)) * sizeof(double);
+    B2N_TRY(b2n_func_smem(ctx, (const void*)(chol_node_kernel<1>), csm));
+    B2N_TRY(b2n_func_smem(ctx, (const void*)(chol_node_kernel<2>), csm));
+    B2N_CUDA(ctx, cudaEventRecord(ctx->ev_side2_go, st));
+    B2N_CUDA(ctx, cudaStreamWaitEvent(ctx->stream_side2, ctx->ev_side2_go, 0));
+    chol_node_kernel<2><<<b.nnodes, 512, csm, ctx->stream_side2>>>(w.na, b.list);
+    B2N_LAUNCH_CHECK(ctx);
+    B2N_CUDA(ctx, cudaEventRecord(ctx->ev_side2, ctx->stream_side2));
+    chol_node_kernel<1><<<b.nnodes, 512, csm, st>>>(w.na, b.list);
+    B2N_LAUNCH_CHECK(ctx);
+    return launch_fmax_finish(w, b, 0, ctx->ev_side2);
 }
 
 // ------------------------------------------------------------------ speculative fit of the root node
@@ -899,28 +890,14 @@ int b2n_spec_root_launch(BoundWork& w, int count, SpecRoot& sp) {
     const int n = w.n;
     const size_t nn = (size_t)n * n;
     sp.launched = false;
-    const int ld = w.na.ld, half = ((n + 1) & ~1) / 2;
-    const size_t small_b = (size_t)(2 * half + 2 * n + 32) * sizeof(double);
-    const size_t eig_smem = small_b + (size_t)2 * n * ld * sizeof(double);
-    if (eig_smem > (size_t)ctx->max_smem_optin) return B2N_OK;          // sliced solver territory: no speculation
-    if (!ctx->stream_side) {
-        int lo = 0, hi = 0;
-        if (cudaDeviceGetStreamPriorityRange(&lo, &hi) != cudaSuccess) { cudaGetLastError(); hi = 0; }
-        B2N_CUDA(ctx, cudaStreamCreateWithPriority(&ctx->stream_side, cudaStreamNonBlocking, hi));
-        B2N_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_side, cudaEventDisableTiming));
-        B2N_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_side_go, cudaEventDisableTiming));
-    }
+    const EigPlan ep = eig_plan(w);
+    if (!ep.smem) return B2N_OK;          // sliced solver territory: no speculation
+    B2N_TRY(side_stream(ctx, ctx->stream_side, ctx->ev_side, ctx->ev_side_go));
     cudaStream_t side = ctx->stream_side;
-    sp.jobs.clear();
-    for (int a = 0; a < count; a += b2n_rows_per_job(w.N)) {
-        JobL j;
-        memset(&j, 0, sizeof(j));
-        j.node = 0; j.r0 = a; j.r1 = std::min(a + b2n_rows_per_job(w.N), count); j.slot = (int)sp.jobs.size(); j.level = 0;
-        sp.jobs.push_back(j);
-    }
+    std::vector<NodeRef> refs(1, b2n_node_ref(0, 0, count, 0));
+    sp.jobs = node_jobs(refs, w.N);
+    sp.ref = refs[0];
     const int njobs = (int)sp.jobs.size();
-    memset(&sp.ref, 0, sizeof(sp.ref));
-    sp.ref.node = 0; sp.ref.start = 0; sp.ref.count = count; sp.ref.slot0 = 0; sp.ref.nslots = njobs; sp.ref.level = 0;
     sp.node0 = 0;
     size_t bytes = 0;
     auto take = [&bytes](size_t b) { const size_t o = bytes; bytes += (b + 255) & ~(size_t)255; return o; };
@@ -946,10 +923,7 @@ int b2n_spec_root_launch(BoundWork& w, int count, SpecRoot& sp) {
     B2N_CUDA(ctx, cudaMemcpyAsync(b + o_ref, &sp.ref, sizeof(NodeRef), cudaMemcpyHostToDevice, side));
     B2N_CUDA(ctx, cudaMemcpyAsync(b + o_list, &sp.node0, sizeof(int), cudaMemcpyHostToDevice, side));
     B2N_CUDA(ctx, cudaMemsetAsync(b + o_stat, 0, sizeof(NodeStat), side));
-    B2N_TRY(b2n_func_smem(ctx, (const void*)(eig_ladder_kernel<true>), eig_smem));
-    const int eig_threads = 32 * std::max(4, std::min(32, (half + 1) / 2));
-    eig_ladder_kernel<true><<<1, eig_threads, eig_smem, side>>>(sp.na, (const int*)(b + o_list), 0, nullptr);
-    B2N_LAUNCH_CHECK(ctx);
+    B2N_TRY(launch_eig(w, ep, sp.na, (const int*)(b + o_list), 1, 0, nullptr, side));
     fmax_partial_kernel<<<dim3(njobs, B2N_FMAX_SUB), 256, (size_t)8 * n * sizeof(double), side>>>(
         w.P, sp.perm, w.N, sp.na, (const JobL*)(b + o_jobs), (double*)(b + o_part));
     B2N_LAUNCH_CHECK(ctx);
@@ -996,45 +970,19 @@ int b2n_read_stats(BoundWork& w, std::vector<NodeStat>& all) {
     return B2N_OK;
 }
 
-// np.mean / np.cov(ddof=1) of one node (rows [0, count) of perm level 0): the moment kernels of b2n_process_nodes
+// np.mean / np.cov(ddof=1) of one node (rows [0, count) of perm level 0): the moment kernels of b2n_fit_nodes
 // without the eigen / fmax stages (used by b2n_friends.cu)
 int b2n_node_moments(BoundWork& w, int count) {
     b2n_ctx* ctx = w.ctx;
-    const int n = w.n;
-    const size_t nn = (size_t)n * n;
-    NodeRef ref;
-    memset(&ref, 0, sizeof(ref));
-    ref.node = 0; ref.start = 0; ref.count = count; ref.level = 0; ref.slot0 = 0;
-    std::vector<JobL> jobs;
-    for (int a = 0; a < count; a += b2n_rows_per_job(w.N)) {
-        JobL j;
-        memset(&j, 0, sizeof(j));
-        j.node = 0; j.r0 = a; j.r1 = std::min(a + b2n_rows_per_job(w.N), count); j.slot = (int)jobs.size(); j.level = 0;
-        jobs.push_back(j);
-    }
-    ref.nslots = (int)jobs.size();
-    const int njobs = (int)jobs.size();
+    std::vector<NodeRef> refs(1, b2n_node_ref(0, 0, count, 0));
+    const std::vector<JobL> jobs = node_jobs(refs, w.N);
     const void *djobs, *drefs;
     B2N_TRY(b2n_in_host(ctx, ctx->scratch4, jobs.data(), jobs.size() * sizeof(JobL), &djobs));
-    B2N_TRY(b2n_in_host(ctx, ctx->scratch5, &ref, sizeof(NodeRef), &drefs));
-    B2N_CUDA(ctx, ctx->scratch1.ensure((size_t)njobs * std::max(nn, (size_t)n) * sizeof(double)));
-    double* partial = ctx->scratch1.as<double>();
-    cudaStream_t st = ctx->stream;
-    colsum_partial_kernel<<<njobs, 256, (size_t)8 * n * sizeof(double), st>>>(w.P, w.perm, w.N, n, (const JobL*)djobs, partial);
-    B2N_LAUNCH_CHECK(ctx);
-    mean_finalize_kernel<<<1, 128, 0, st>>>((const NodeRef*)drefs, n, partial, w.na.mean);
-    B2N_LAUNCH_CHECK(ctx);
-    const int ntile = (n + B2N_TILE - 1) / B2N_TILE;
-    cov_partial_kernel<<<dim3(njobs, ntile * (ntile + 1) / 2), 256, 0, st>>>(w.P, w.perm, w.N, n, (const JobL*)djobs,
-                                                                            w.na.mean, partial, ntile);
-    B2N_LAUNCH_CHECK(ctx);
-    cov_finalize_kernel<<<dim3(1, (unsigned)std::min<size_t>((nn + 255) / 256, 64)), 256, 0, st>>>(
-        (const NodeRef*)drefs, n, partial, w.na.covraw);
-    B2N_LAUNCH_CHECK(ctx);
-    return B2N_OK;
+    B2N_TRY(b2n_in_host(ctx, ctx->scratch5, refs.data(), sizeof(NodeRef), &drefs));
+    return launch_moments(w, NodeBatch{1, (int)jobs.size(), (const JobL*)djobs, (const NodeRef*)drefs, nullptr});
 }
 
-static int init_identity_perm(BoundWork& w) {
+int b2n_init_identity_perm(BoundWork& w) {
     std::vector<int> id(w.N);
     for (int64_t i = 0; i < w.N; i++) id[i] = (int)i;
     B2N_CUDA(w.ctx, cudaMemcpyAsync(w.perm, id.data(), w.N * sizeof(int), cudaMemcpyHostToDevice, w.ctx->stream));
@@ -1042,8 +990,7 @@ static int init_identity_perm(BoundWork& w) {
 }
 
 // copy node `node` arrays to caller outputs (device or host according to pointer mode)
-static int emit_node(BoundWork& w, int node, int k, double* ctr, double* cov, double* am, double* axes,
-                     double* axlens) {
+int b2n_emit_node(BoundWork& w, int node, int k, double* ctr, double* cov, double* am, double* axes, double* axlens) {
     b2n_ctx* ctx = w.ctx;
     const size_t n = w.n, nn = n * n;
     const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
@@ -1055,11 +1002,6 @@ static int emit_node(BoundWork& w, int node, int k, double* ctr, double* cov, do
     return B2N_OK;
 }
 
-int b2n_emit_node(BoundWork& w, int node, int k, double* ctr, double* cov, double* am, double* axes, double* axlens) {
-    return emit_node(w, node, k, ctr, cov, am, axes, axlens);
-}
-int b2n_init_identity_perm(BoundWork& w) { return init_identity_perm(w); }
-
 extern "C" int b2n_bounding_ellipsoid(b2n_ctx* ctx, const double* points, int64_t N, int32_t n, double* ctr,
                                       double* cov, double* am, double* axes, double* axlens, double* logvol,
                                       uint32_t* warn) {
@@ -1070,15 +1012,12 @@ extern "C" int b2n_bounding_ellipsoid(b2n_ctx* ctx, const double* points, int64_
     B2N_TRY(b2n_in(ctx, ctx->in0, points, (size_t)N * n * sizeof(double), &dP));
     BoundWork w;
     B2N_TRY(b2n_boundwork_init(ctx, w, (const double*)dP, N, n, 1));
-    B2N_TRY(init_identity_perm(w));
-    std::vector<NodeRef> refs(1);
-    memset(&refs[0], 0, sizeof(NodeRef));
-    refs[0].node = 0; refs[0].start = 0; refs[0].count = (int)N; refs[0].level = 0;
+    B2N_TRY(b2n_init_identity_perm(w));
     std::vector<NodeStat> hs;
-    B2N_TRY(b2n_process_nodes(w, refs, hs));
+    B2N_TRY(b2n_fit_nodes(w, std::vector<NodeRef>(1, b2n_node_ref(0, 0, (int)N, 0)), hs));
     if (warn) *warn = hs[0].fallback ? B2N_WARN_IDENTITY_FALLBACK : 0u;
     if (hs[0].error) return hs[0].error;
-    B2N_TRY(emit_node(w, 0, 0, ctr, cov, am, axes, axlens));
+    B2N_TRY(b2n_emit_node(w, 0, 0, ctr, cov, am, axes, axlens));
     if (logvol) {
         if (ctx->ptr_mode == B2N_PTR_DEVICE)
             B2N_CUDA(ctx, cudaMemcpyAsync(logvol, &hs[0].logvol, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -1100,10 +1039,10 @@ extern "C" int b2n_moments(b2n_ctx* ctx, const double* points, int64_t N, int32_
     B2N_TRY(b2n_in(ctx, ctx->in0, points, (size_t)N * n * sizeof(double), &dP));
     BoundWork w;
     B2N_TRY(b2n_boundwork_init(ctx, w, (const double*)dP, N, n, 1));
-    B2N_TRY(init_identity_perm(w));
+    B2N_TRY(b2n_init_identity_perm(w));
     B2N_TRY(b2n_node_moments(w, (int)N));
     if (N == 1) B2N_CUDA(ctx, cudaMemsetAsync(w.na.covraw, 0, (size_t)n * n * sizeof(double), ctx->stream));   // (ddof = 1)
-    B2N_TRY(emit_node(w, 0, 0, mean, nullptr, nullptr, nullptr, nullptr));
+    B2N_TRY(b2n_emit_node(w, 0, 0, mean, nullptr, nullptr, nullptr, nullptr));
     const cudaMemcpyKind kind = ctx->ptr_mode == B2N_PTR_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     B2N_CUDA(ctx, cudaMemcpyAsync(cov, w.na.covraw, (size_t)n * n * sizeof(double), kind, ctx->stream));
     B2N_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1126,16 +1065,14 @@ extern "C" int b2n_improve_covar(b2n_ctx* ctx, const double* covar, int32_t n, d
     const int zero = 0;
     const void* dlist;
     B2N_TRY(b2n_in_host(ctx, ctx->work0, &zero, sizeof(int), &dlist));
-    const int ld = w.na.ld, half = ((n + 1) & ~1) / 2;
-    const size_t small_b = (size_t)(2 * half + 2 * n + 32) * sizeof(double);
-    const size_t mats_b = (size_t)2 * n * ld * sizeof(double);
-    const int use_smem = small_b + mats_b <= (size_t)ctx->max_smem_optin ? 1 : 0;
+    const EigPlan ep = eig_plan(w);
     NodeStat hs;
     memset(&hs, 0, sizeof(hs));
     int sliced = 0;
-    if (!use_smem) {
+    if (!ep.smem) {
         B2N_TRY(b2n_eig_sliced(w, (const int*)dlist, 1, 0, 0, &sliced));
-        for (int attempt = 1; sliced && attempt <= 100; attempt++) {        // one decomposition per launch
+        // one decomposition per launch; attempt 99 is the 100th, which ends the ladder (eig_check_kernel)
+        for (int attempt = 1; sliced && attempt <= 100; attempt++) {
             B2N_CUDA(ctx, cudaStreamSynchronize(st));
             B2N_CUDA(ctx, b2n_copy_sync(ctx, &hs, w.na.stat, sizeof(NodeStat), cudaMemcpyDeviceToHost));
             if (!hs.retry) break;
@@ -1144,27 +1081,18 @@ extern "C" int b2n_improve_covar(b2n_ctx* ctx, const double* covar, int32_t n, d
         }
     }
     if (!sliced) {
-        const size_t eig_smem = small_b + (use_smem ? mats_b : 0);
         double* gwork = nullptr;
-        if (!use_smem) {
-            B2N_CUDA(ctx, ctx->scratch2.ensure(mats_b));
+        if (!ep.smem) {
+            B2N_CUDA(ctx, ctx->scratch2.ensure(ep.gwork_bytes));
             gwork = ctx->scratch2.as<double>();
         }
-        const int ethreads = 32 * std::max(4, std::min(32, (half + 1) / 2));
-        if (use_smem) {
-            B2N_TRY(b2n_func_smem(ctx, (const void*)(eig_ladder_kernel<true>), (size_t)(eig_smem)));
-            eig_ladder_kernel<true><<<1, ethreads, eig_smem, st>>>(w.na, (const int*)dlist, 0, gwork);
-        } else {
-            B2N_TRY(b2n_func_smem(ctx, (const void*)(eig_ladder_kernel<false>), (size_t)(eig_smem)));
-            eig_ladder_kernel<false><<<1, ethreads, eig_smem, st>>>(w.na, (const int*)dlist, 0, gwork);
-        }
-        B2N_LAUNCH_CHECK(ctx);
+        B2N_TRY(launch_eig(w, ep, w.na, (const int*)dlist, 1, 0, gwork, st));
     }
     B2N_CUDA(ctx, cudaStreamSynchronize(st));
     B2N_CUDA(ctx, b2n_copy_sync(ctx, &hs, w.na.stat, sizeof(NodeStat), cudaMemcpyDeviceToHost));
     if (good) *good = hs.good;
     if (warn) *warn = hs.fallback ? B2N_WARN_IDENTITY_FALLBACK : 0u;
-    B2N_TRY(emit_node(w, 0, 0, nullptr, cov_out, am, axes, nullptr));
+    B2N_TRY(b2n_emit_node(w, 0, 0, nullptr, cov_out, am, axes, nullptr));
     B2N_CUDA(ctx, cudaStreamSynchronize(st));
     return B2N_OK;
 }

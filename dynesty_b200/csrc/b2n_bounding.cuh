@@ -34,12 +34,6 @@ struct NodeStat {
     double logvol;
 };
 
-struct MomentJob {   // one CTA-sized slice of one node
-    int node;        // index into the node arrays
-    int r0, r1;      // rows [r0, r1) of perm
-    int slot;        // partial-result slot
-};
-
 struct NodeRef {     // per-node view used by finalize kernels
     int node;
     int start, count;
@@ -71,18 +65,21 @@ struct BoundWork {
 };
 #ifdef __cplusplus
 #include <vector>
+static inline NodeRef b2n_node_ref(int node, int start, int count, int level) {
+    return NodeRef{node, start, count, 0, 0, level};
+}
 int b2n_boundwork_init(b2n_ctx* ctx, BoundWork& w, const double* dP, int64_t N, int n, int cap);
-// candidate = false: the full path (eigen-decomposition + repair ladder).  candidate = true: nodes that
-// are only CANDIDATES of the multi-ellipsoid tree (bounding.py:1464-1563 evaluates every candidate but
-// returns few): Cholesky-based precision / log-volume + power-iteration major axis, see chol_node_kernel.
-// defer (candidates only): return after the launches, without the host read-back of the stats -> b2n_read_stats.
-int b2n_process_nodes(BoundWork& w, const std::vector<NodeRef>& refs, std::vector<NodeStat>& stats,
-                      bool candidate = false, bool defer = false);
+// The full fit (eigen-decomposition + repair ladder) of every node; synchronises and returns the nodes' stats.
+int b2n_fit_nodes(BoundWork& w, const std::vector<NodeRef>& refs, std::vector<NodeStat>& stats);
+// Nodes that are only CANDIDATES of the multi-ellipsoid tree (bounding.py:1464-1563 evaluates every candidate but
+// returns few): Cholesky-based precision / log-volume + major axis, see chol_node_kernel.  Enqueued only: the
+// stats are read later with b2n_read_stats.
+int b2n_fit_candidates(BoundWork& w, const std::vector<NodeRef>& refs);
 int b2n_read_stats(BoundWork& w, std::vector<NodeStat>& all);
-// speculative eigen fit of the root node on the context's side stream (b2n_bounding.cu)
-struct JobL {   // MomentJob + perm level
+struct JobL {   // one CTA-sized slice of one node: rows [r0, r1) of perm level `level`, partial-result slot `slot`
     int node, r0, r1, slot, level, pad0, pad1, pad2;
 };
+// speculative eigen fit of the root node on the context's side stream (b2n_bounding.cu)
 struct SpecRoot {
     bool launched = false;
     NodeArrays na;               // shadow arrays of node 0 (mean / covraw alias the main arrays)

@@ -343,20 +343,17 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
     HNode root;
     root.start = 0; root.count = count; root.level = 0; root.child[0] = root.child[1] = -1; root.split[0] = root.split[1] = -1; root.logvol = 0;
     tree.push_back(root);
-    std::vector<NodeRef> refs(1);
-    memset(&refs[0], 0, sizeof(NodeRef));
-    refs[0].node = 0; refs[0].start = 0; refs[0].count = count; refs[0].level = 0;
+    const std::vector<NodeRef> refs(1, b2n_node_ref(0, 0, count, 0));
     std::vector<NodeStat> hs;
     // fast: the candidates' stats are read ONCE, after the expansion (nothing on the host needs them earlier:
     // the k-means start centres, the partitions and the children's fits read the node arrays on the device) --
     // a level's launches queue behind the previous level's without a host round trip
-    const char* denv = getenv("B2N_BOUND_DEFER");
-    const bool defer = fast && !(denv && denv[0] == '0');
-    B2N_TRY(b2n_process_nodes(w, refs, hs, fast, defer));
-    if (!defer) {
-        if (fast && (hs[0].suspect || hs[0].pad)) return B2N_RETRY_FULL;
+    if (fast) {
+        B2N_TRY(b2n_fit_candidates(w, refs));
+    } else {
+        B2N_TRY(b2n_fit_nodes(w, refs, hs));
         if (hs[0].fallback && warn) *warn |= B2N_WARN_IDENTITY_FALLBACK;
-        if (hs[0].error) return fast ? B2N_RETRY_FULL : hs[0].error;
+        if (hs[0].error) return hs[0].error;
         tree[0].logvol = hs[0].logvol;
     }
     // the root's full (eigen) fit, speculatively, on the side stream while the tree is expanded (b2n_bounding.cu);
@@ -366,11 +363,7 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
         explicit SpecScope(b2n_ctx* ctx) : c(ctx) {}
         ~SpecScope() { b2n_spec_root_wait(c, sp); }
     } spec(ctx);
-    {
-        const char* senv = getenv("B2N_BOUND_SPEC");
-        if (fast && count >= 4 * n && count == (int)w.N && !(senv && senv[0] == '0'))
-            B2N_TRY(b2n_spec_root_launch(w, count, spec.sp));
-    }
+    if (fast && count >= 4 * n && count == (int)w.N) B2N_TRY(b2n_spec_root_launch(w, count, spec.sp));
 
     // scale = std of the ROOT points, reused at every depth (:1503-1504, 1548-1549)
     B2N_CUDA(ctx, ctx->work1.ensure((size_t)n * sizeof(double)));
@@ -403,20 +396,15 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
     // rows a CTA may stage in shared memory (its eighth of the largest node of a level), within half an SM's
     // shared memory so that the chain kernels of other replicas keep their place next to it
     const size_t km_room = std::min((size_t)ctx->max_smem_optin, (size_t)120 * 1024);
-    int km_stage_max = km_room > km_base ? (int)((km_room - km_base) / ((size_t)(n | 1) * sizeof(double) + 1)) : 0;
-    if (const char* e = getenv("B2N_KM_STAGE")) if (e[0] == '0') km_stage_max = 0;     // A/B switch: every row from L2, as before
+    const int km_stage_max = km_room > km_base ? (int)((km_room - km_base) / ((size_t)(n | 1) * sizeof(double) + 1)) : 0;
 
     while (!frontier.empty()) {
         std::vector<int> split;
         for (int id : frontier)
             if (tree[id].count >= 2 * min_size) split.push_back(id);      // :1493
         if (split.empty()) break;
-        std::vector<NodeRef> srefs(split.size());
-        for (size_t i = 0; i < split.size(); i++) {
-            memset(&srefs[i], 0, sizeof(NodeRef));
-            srefs[i].node = split[i]; srefs[i].start = tree[split[i]].start; srefs[i].count = tree[split[i]].count;
-            srefs[i].level = cur;
-        }
+        std::vector<NodeRef> srefs;
+        for (int id : split) srefs.push_back(b2n_node_ref(id, tree[id].start, tree[id].count, cur));
         const void* drefs;
         B2N_TRY(b2n_in_host(ctx, ctx->scratch5, srefs.data(), srefs.size() * sizeof(NodeRef), &drefs));
         const int* pin = w.perm + (size_t)cur * w.N;
@@ -451,18 +439,16 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
                 ch.count = k ? c1 : c0;
                 ch.level = cur; ch.child[0] = ch.child[1] = -1; ch.split[0] = ch.split[1] = -1; ch.logvol = 0;
                 tree[id].child[k] = (int)tree.size();
-                NodeRef r;
-                memset(&r, 0, sizeof(r));
-                r.node = (int)tree.size(); r.start = ch.start; r.count = ch.count; r.level = cur;
-                crefs.push_back(r);
+                crefs.push_back(b2n_node_ref((int)tree.size(), ch.start, ch.count, cur));
                 next.push_back((int)tree.size());
                 tree.push_back(ch);
             }
         }
-        if (!crefs.empty()) {
-            B2N_TRY(b2n_process_nodes(w, crefs, hs, fast, defer));
-            for (size_t i = 0; !defer && i < crefs.size(); i++) {
-                if (fast && (hs[i].suspect || hs[i].pad || hs[i].error)) return B2N_RETRY_FULL;
+        if (fast) {
+            B2N_TRY(b2n_fit_candidates(w, crefs));
+        } else if (!crefs.empty()) {
+            B2N_TRY(b2n_fit_nodes(w, crefs, hs));
+            for (size_t i = 0; i < crefs.size(); i++) {
                 if (hs[i].fallback && warn) *warn |= B2N_WARN_IDENTITY_FALLBACK;
                 if (hs[i].error) return hs[i].error;
                 tree[crefs[i].node].logvol = hs[i].logvol;
@@ -470,7 +456,7 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
         }
         frontier = next;
     }
-    if (defer) {
+    if (fast) {
         std::vector<NodeStat> all;
         B2N_TRY(b2n_read_stats(w, all));
         for (size_t id = 0; id < tree.size(); id++) {
@@ -492,13 +478,9 @@ static int decompose(BoundWork& w, int count, std::vector<HNode>& tree, std::vec
         // the accepted leaves get the full fit (eigen-decomposition: axes, axlens, and the reference's exact
         // ladder / rescale); a leaf's points are the segment [start, start+count) of EITHER index buffer as a
         // set (partitions only permute inside segments), so the last buffer serves all of them
-        std::vector<NodeRef> lrefs(leaves.size());
-        for (size_t k = 0; k < leaves.size(); k++) {
-            memset(&lrefs[k], 0, sizeof(NodeRef));
-            lrefs[k].node = leaves[k]; lrefs[k].start = tree[leaves[k]].start; lrefs[k].count = tree[leaves[k]].count;
-            lrefs[k].level = cur;
-        }
-        B2N_TRY(b2n_process_nodes(w, lrefs, hs, false));
+        std::vector<NodeRef> lrefs;
+        for (int id : leaves) lrefs.push_back(b2n_node_ref(id, tree[id].start, tree[id].count, cur));
+        B2N_TRY(b2n_fit_nodes(w, lrefs, hs));
         for (size_t k = 0; k < leaves.size(); k++) {
             if (hs[k].fallback && warn) *warn |= B2N_WARN_IDENTITY_FALLBACK;
             if (hs[k].error) return hs[k].error;
@@ -716,12 +698,9 @@ extern "C" int b2n_bootstrap_expand(b2n_ctx* ctx, const double* points, int64_t 
         if (multi) {
             B2N_TRY(decompose(w, (int)n_in, tree, leaves, level, nullptr));
         } else {
-            std::vector<NodeRef> refs(1);
-            memset(&refs[0], 0, sizeof(NodeRef));
-            refs[0].node = 0; refs[0].start = 0; refs[0].count = (int)n_in; refs[0].level = 0;
             std::vector<NodeStat> hs;
             if (n_in == 1) return B2N_ERR_SINGLE_POINT;
-            B2N_TRY(b2n_process_nodes(w, refs, hs));
+            B2N_TRY(b2n_fit_nodes(w, std::vector<NodeRef>(1, b2n_node_ref(0, 0, (int)n_in, 0)), hs));
             if (hs[0].error) return hs[0].error;
             leaves.assign(1, 0);
         }

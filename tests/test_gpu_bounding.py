@@ -8,7 +8,7 @@ condition number); axes through axes @ axes.T = cov and sorted axis lengths."""
 import numpy as np
 import pytest
 
-from dynesty_b200 import ops
+from dynesty_b200 import _lib, ops
 from helpers import close, SEED
 from oracle import bounding as OB, philox
 
@@ -144,25 +144,20 @@ def test_bootstrap_expand_golden(golden, multi):
     np.testing.assert_allclose(got, g['boot_%d_expand' % multi], rtol=1e-8)
 
 
-@pytest.mark.parametrize('case', ['gauss2000x50', 'clusters4000x25', 'grid'])
+@pytest.mark.parametrize('case', ['gauss2000x50', 'clusters4000x25', 'two20000x8', 'illcond600x12', 'grid'])
 def test_candidate_path_equals_eigen_path(case, monkeypatch):
     """The candidates of the multi-ellipsoid tree go through the Cholesky / matrix-squaring kernel
     (chol_node_kernel), only the accepted leaves through the eigen path; B2N_BOUND_FAST=0 forces the eigen
     path for every node.  Same tree, same leaves: nells equal, centres / covariances / log-volumes to
     round-off (the leaf fits see the points in a different order), every point inside its ellipsoid.
-    'grid' has exactly degenerate spectra: the candidate path cannot certify its nodes and must fall back."""
-    rng = np.random.default_rng(SEED)
-    if case == 'gauss2000x50':
-        Cm = np.full((50, 50), 0.4)
-        np.fill_diagonal(Cm, 1.0)
-        pts = 0.5 + 0.02 * rng.standard_normal((2000, 50)) @ np.linalg.cholesky(Cm).T
-    elif case == 'clusters4000x25':
-        ctrs = 0.2 + 0.6 * rng.random((8, 25))
-        pts = np.concatenate([c + 0.01 * rng.standard_normal((500, 25)) for c in ctrs])
-    else:
+    'two20000x8' has two leaves; 'illcond600x12' and 'grid' (exactly degenerate spectra) have nodes the
+    candidate path cannot certify: it must fall back."""
+    if case == 'grid':
         g1 = np.linspace(0.2, 0.8, 5)
         pts = np.array(np.meshgrid(g1, g1, g1)).reshape(3, -1).T
         pts = np.concatenate([pts, pts + 1e-3, pts - 1e-3, pts + 2e-3])
+    else:
+        pts = _clouds(case)
     monkeypatch.setenv('B2N_BOUND_FAST', '0')
     slow = ops.multi_decompose(pts)
     monkeypatch.setenv('B2N_BOUND_FAST', '1')
@@ -200,58 +195,81 @@ def _clouds(case):
 @pytest.mark.parametrize('case', ['gauss2000x50', 'clusters4000x25', 'two20000x8', 'illcond600x12'])
 def test_speculative_root_fit_equals_refit(case, monkeypatch):
     """b2n_spec_root_*: the root's eigen fit runs on a side stream while the candidate tree is expanded and is
-    adopted when the root is the accepted leaf (B2N_BOUND_SPEC=0: the ordinary re-fit after the tree).  Same
-    kernels on the same rows in a different ORDER (identity against the last permutation): equal to round-off."""
+    adopted when the root is the accepted leaf (gauss2000x50; the others have several leaves or a root whose
+    covariance needs the repair ladder, and are re-fitted after the tree).  The adopted fit runs the kernels of
+    bounding_ellipsoid on the same rows in the same order: equal to the bit.  Every case is reproducible call to
+    call."""
     pts = _clouds(case)
     monkeypatch.setenv('B2N_BOUND_FAST', '1')           # attempt the candidate path whatever this context saw before
-    monkeypatch.setenv('B2N_BOUND_SPEC', '0')
-    a = ops.multi_decompose(pts)
-    monkeypatch.setenv('B2N_BOUND_SPEC', '1')
     b = ops.multi_decompose(pts)
-    b2 = ops.multi_decompose(pts)                       # and reproducible call to call
-    assert a['nells'] == b['nells'] == b2['nells']
-    assert np.array_equal(a['labels'], b['labels'])
-    for k in ('ctrs', 'covs', 'ams', 'axes', 'logvols'):
+    b2 = ops.multi_decompose(pts)
+    assert b['nells'] == b2['nells']
+    for k in ('labels', 'ctrs', 'covs', 'ams', 'axes', 'logvols'):
         assert np.array_equal(b[k], b2[k]), k
-    close(b['ctrs'], a['ctrs'], rtol=1e-12)
-    close(b['covs'], a['covs'], rtol=1e-9)
-    close(b['logvols'], a['logvols'], rtol=1e-11)
-    close(b['ams'], a['ams'], rtol=1e-6 if case.startswith('illcond') else 1e-8)
+    if case == 'gauss2000x50':
+        a = ops.bounding_ellipsoid(pts)
+        assert b['nells'] == 1
+        for k, kb in (('ctr', 'ctrs'), ('cov', 'covs'), ('am', 'ams'), ('axes', 'axes'), ('axlens', 'axlens')):
+            assert np.array_equal(b[kb][0], a[k]), k
+        assert b['logvols'][0] == a['logvol']
     for k in range(b['nells']):
         close(b['axes'][k] @ b['axes'][k].T, b['covs'][k], rtol=1e-9)
     mask = ops.membership(pts, b['ctrs'], b['ams'])[0]
     assert mask[np.arange(len(pts)), b['labels']].all()
 
 
-@pytest.mark.parametrize('case', ['gauss2000x50', 'clusters4000x25', 'two20000x8'])
-@pytest.mark.parametrize('switch', ['B2N_KM_STAGE', 'B2N_CHOL_SPLIT', 'B2N_BOUND_DEFER'])
-def test_update_variants_equal(case, switch, monkeypatch):
-    """Re-arrangements of the update.  Bit for bit: (i) B2N_CHOL_SPLIT, the two halves of the candidate fit (Cholesky /
-    major axis) as two launches on two streams; (ii) B2N_BOUND_DEFER, the candidates' stats read back once after the
-    expansion instead of once per level.  Same splits, sums in another order: (iii) B2N_KM_STAGE, the k-means CTAs
-    stage their rows in shared memory and run the thread-per-row Lloyd iteration (0: warp per row from L2;
-    two20000x8: the root's CTAs hold 2500 rows each, more than the stage takes, deeper nodes fit)."""
-    pts = _clouds(case)
-    monkeypatch.setenv('B2N_BOUND_FAST', '1')
-    monkeypatch.setenv('B2N_BOUND_SPEC', '0')
-    monkeypatch.setenv(switch, '0')
-    a = ops.multi_decompose(pts)
-    monkeypatch.setenv(switch, '1')
-    b = ops.multi_decompose(pts)
-    assert a['nells'] == b['nells'] and a['warn'] == b['warn']
-    if switch == 'B2N_KM_STAGE':
-        # leaves come out in tree order; a centroid that differs in its last bits may flip a point exactly on a
-        # bisecting plane, nothing else
-        assert np.mean(a['labels'] != b['labels']) < 1e-3
-        close(b['ctrs'], a['ctrs'], rtol=1e-3 if np.any(a['labels'] != b['labels']) else 1e-12)
-        close(b['logvols'], a['logvols'], rtol=1e-2 if np.any(a['labels'] != b['labels']) else 1e-11)
-    else:
-        for k in ('labels', 'ctrs', 'covs', 'ams', 'axes', 'axlens', 'logvols'):
-            assert np.array_equal(a[k], b[k]), k
-    if case == 'clusters4000x25':
-        assert b['nells'] == 8
-    mask = ops.membership(pts, b['ctrs'], b['ams'])[0]
-    assert mask[np.arange(len(pts)), b['labels']].all()
+def _indefinite(n):
+    """A symmetric matrix with two negative eigenvalues: improve_covar runs its repair ladder."""
+    rng = np.random.default_rng(n)
+    A = rng.standard_normal((n, n))
+    lam, V = np.linalg.eigh(A @ A.T / n)
+    lam[:2] = -lam[:2]
+    M = (V * lam) @ V.T
+    return 0.5 * (M + M.T)
+
+
+def _line150():
+    """Collinear points in 150 dimensions: the sliced eigensolver's repair ladder and the second pass."""
+    x = np.random.default_rng(1).random(200)
+    return 0.5 + (x[:, None] - 0.5) * np.ones((1, 150)) * 0.2
+
+
+# One call of each bound-update entry point, on a fresh context (no state carried over, such as the eigen path taken
+# for a while after a candidate could not be certified).  n = 50 / 40 keep the eigen solve in one CTA's shared
+# memory; n = 150 takes the sliced solver.
+LAUNCH_CALLS = {
+    'bounding_ellipsoid-n50': lambda ctx: ops.bounding_ellipsoid(_clouds('gauss2000x50'), ctx=ctx),
+    'bounding_ellipsoid-n150': lambda ctx: ops.bounding_ellipsoid(_line150(), ctx=ctx),
+    'improve_covar-n40': lambda ctx: ops.improve_covar(_indefinite(40), ctx=ctx),
+    'improve_covar-n150': lambda ctx: ops.improve_covar(_indefinite(150), ctx=ctx),
+    'moments-n50': lambda ctx: ops.moments(_clouds('gauss2000x50'), ctx=ctx),
+    'moments-n150': lambda ctx: ops.moments(_line150(), ctx=ctx),
+    'multi_decompose-gauss2000x50': lambda ctx: ops.multi_decompose(_clouds('gauss2000x50'), ctx=ctx),
+    'multi_decompose-clusters4000x25': lambda ctx: ops.multi_decompose(_clouds('clusters4000x25'), ctx=ctx),
+    'multi_decompose-two20000x8': lambda ctx: ops.multi_decompose(_clouds('two20000x8'), ctx=ctx),
+    'multi_decompose-illcond600x12': lambda ctx: ops.multi_decompose(_clouds('illcond600x12'), ctx=ctx),
+    'bootstrap_expand-single': lambda ctx: ops.bootstrap_expand(_clouds('clusters4000x25'), 0, 2, SEED, 1000, ctx=ctx),
+    'bootstrap_expand-multi': lambda ctx: ops.bootstrap_expand(_clouds('clusters4000x25'), 1, 2, SEED, 1000, ctx=ctx),
+    'friends_update': lambda ctx: ops.friends_update(_clouds('gauss2000x50'), 'balls', ctx=ctx),
+}
+LAUNCHES = {'bounding_ellipsoid-n50': 7, 'bounding_ellipsoid-n150': 24, 'improve_covar-n40': 1,
+            'improve_covar-n150': 9, 'moments-n50': 4, 'moments-n150': 4, 'multi_decompose-gauss2000x50': 55,
+            'multi_decompose-clusters4000x25': 99, 'multi_decompose-two20000x8': 137,
+            'multi_decompose-illcond600x12': 137, 'bootstrap_expand-single': 18, 'bootstrap_expand-multi': 141,
+            'friends_update': 12}
+
+
+@pytest.mark.parametrize('call', sorted(LAUNCH_CALLS))
+def test_bound_update_launches(call, monkeypatch):
+    """Kernel launches per call of the bound-update entry points (B2N_BOUND_FAST unset: the default path)."""
+    monkeypatch.delenv('B2N_BOUND_FAST', raising=False)
+    ctx = _lib.Context(0)
+    try:
+        before = ctx.launch_count()
+        LAUNCH_CALLS[call](ctx)
+        assert ctx.launch_count() - before == LAUNCHES[call]
+    finally:
+        ctx.close()
 
 
 # ---- improve_covar_mat on its own (b2n_improve_covar): the reference's test matrices (tests/test_ellipsoid.py:242-255)

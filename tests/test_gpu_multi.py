@@ -33,7 +33,7 @@ def _optin():
     return int(torch.cuda.get_device_properties(0).shared_memory_per_block_optin)
 
 
-# ---- the host's formulas (b2n_multi.cu decompose / multi_run, b2n_bounding.cu b2n_process_nodes, b2n_eig_sliced.cu)
+# ---- the host's formulas (b2n_multi.cu decompose / multi_run, b2n_bounding.cu b2n_fit_nodes, b2n_eig_sliced.cu)
 def km_stage_max(n, optin):
     nw = 16
     while (6 * n + nw * 2 * n) * 8 + nw * 2 * 4 > optin and nw > 1:
