@@ -51,6 +51,14 @@ class ChainArgs(C.Structure):
                 ('scale', C.c_double), ('seed', C.c_uint64), ('chain0', C.c_uint64)]
 
 
+class RwalkState(C.Structure):
+    """b2n_rwalk_state: the device buffers of a stepped random walk (b2n_rwalk_step / b2n_ns_rwalk_step)."""
+    _fields_ = [('u_prop', C.c_void_p), ('v_prop', C.c_void_p), ('logl_prop', C.c_void_p), ('u_start', C.c_void_p),
+                ('v_start', C.c_void_p), ('logl_start', C.c_void_p), ('tick', C.c_void_p), ('in_cube', C.c_void_p),
+                ('dimflags', C.c_void_p), ('order', C.c_void_p), ('cta', C.c_void_p), ('ncta', C.c_int32),
+                ('reserved', C.c_int32)]
+
+
 class NsConfig(C.Structure):
     _fields_ = [('nlive', C.c_int32), ('ndim', C.c_int32), ('ncdim', C.c_int32), ('batch', C.c_int32),
                 ('sampler', C.c_int32), ('steps', C.c_int32), ('model_id', C.c_int32),
@@ -115,6 +123,7 @@ SYMBOLS = {
                                        _P, _P]),
     'b2n_bound_set': (C.c_int, [_P, _I, _I, _P, _P, _P, _P]),
     'b2n_rwalk_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _P, _P, _P, _P, _P, _P]),
+    'b2n_rwalk_step': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _I, C.POINTER(RwalkState), _P, _P, _P, _P, _P, _P]),
     'b2n_rslice_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_slice_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_unitcube_batch': (C.c_int, [_P, C.POINTER(ChainArgs), _P, _P, _P, _P, _P]),
@@ -132,6 +141,8 @@ SYMBOLS = {
     'b2n_ns_set_state': (C.c_int, [_P, _P, _P, _P, _D, _D, _D, _L, _L, _D]),
     'b2n_ns_run': (C.c_int, [_P, _I, _I, C.POINTER(NsStatus)]),
     'b2n_ns_status_get': (C.c_int, [_P, C.POINTER(NsStatus)]),
+    'b2n_ns_step': (C.c_int, [_P, _I]),
+    'b2n_ns_rwalk_step': (C.c_int, [_P, _I, C.POINTER(RwalkState)]),
     'b2n_ns_set_counters': (C.c_int, [_P, _L, _L, _I]),
     'b2n_ns_bound_updated': (C.c_int, [_P]),
     'b2n_ns_update_bound': (C.c_int, [_P, _I, _D, _P, _P, _P]),
@@ -216,6 +227,8 @@ class Context:
         self.h = h
         self.device = device
         self.mode = PTR_HOST
+        self.stream = None                   # the cudaStream_t given to set_stream (None: the context's own)
+        self.ns_stepped = None               # (batch, ndim, walks, dimflags) of a device run with stepped chains
 
     def close(self):
         if getattr(self, 'h', None):
@@ -239,6 +252,7 @@ class Context:
 
     def set_stream(self, stream):
         self.check(self.lib.b2n_set_stream(self.h, stream))
+        self.stream = stream
 
     def set_pointer_mode(self, mode):
         self.check(self.lib.b2n_set_pointer_mode(self.h, mode))

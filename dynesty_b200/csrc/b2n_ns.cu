@@ -31,6 +31,7 @@
 // flag in HBM; the remaining enqueued rounds return at once and the host picks the flag up at its
 // next status read.
 #include "b2n_device.cuh"
+#include "b2n_rwalk_step.cuh"
 #include <algorithm>
 #include <math_constants.h>
 
@@ -625,12 +626,48 @@ static size_t ns_commit_smem(const NsDev& d) {
 }
 static size_t ns_sort_smem(const NsDev& d) { return (size_t)d.Npad * 12 + 64; }
 
+// Per-run launch parameters of the round kernels from the resident bound and the chain kernel's plan; raises the
+// step kernel's shared-memory limit.  *smem: its dynamic shared memory.
+static int ns_prepare(b2n_ctx* ctx, b2n_ns* ns, size_t* smem_out) {
+    NsDev& d = ns->d;
+    if (ns->phase == 0) {            // unit-cube rounds: no bound yet
+        d.Kell = 1;
+        d.ctrs = d.ams = d.logvols = nullptr;
+    } else {
+        if (ctx->bK < 1 || ctx->bn != d.nc) return b2n_fail(ctx, B2N_ERR_ARG, "resident bound missing or of wrong dimension (b2n_bound_set)");
+        if (!ctx->b_ctrs.p || !ctx->b_ams.p || !ctx->b_logvols.p || ctx->h_logvols.empty())
+            return b2n_fail(ctx, B2N_ERR_ARG, "b2n_ns_run needs the full resident bound (ctrs, ams, logvols)");
+        d.Kell = ctx->bK;
+        d.ctrs = ctx->b_ctrs.as<double>(); d.ams = ctx->b_ams.as<double>(); d.logvols = ctx->b_logvols.as<double>();
+    }
+    d.strict = ns->cfg.strict_contains;
+    if ((size_t)d.K / 1 + (size_t)d.Kell + 8 > (size_t)d.K + (size_t)d.N + 8)
+        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "too many ellipsoids for the round worklist");
+    if (ns->cfg.model_id < 0) {                          // chains per CTA the chain kernel plans for
+        int warps;
+        size_t chain_smem;
+        B2N_TRY(b2n_rwalk_step_plan(ctx, d.K, d.n, &d.cpc, &warps, &chain_smem));
+    } else {
+        B2N_TRY(ns_chain_call(ctx, ns, true));
+        d.cpc = ctx->dyn.cpc;
+    }
+    const size_t smem = std::max(ns_propose_smem(d), ns_commit_smem(d));
+    if (smem + 2048 > (size_t)ctx->max_smem_optin)
+        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "nlive / batch too large for the one-CTA kernels of b2n_ns_run");
+    B2N_TRY(b2n_func_smem(ctx, (const void*)(ns_step_kernel), (size_t)(smem)));
+    *smem_out = smem;
+    return B2N_OK;
+}
+
 extern "C" {
 
 int b2n_ns_create(b2n_ctx* ctx, const b2n_ns_config* c, int64_t dead_capacity) {
     if (!ctx || !c) return B2N_ERR_ARG;
-    if (c->model_id < 0 || c->model_id >= (int)ctx->models.size()) return B2N_ERR_ARG;
-    const int n = ctx->models[c->model_id].ndim;
+    const bool stepped = c->model_id == -1;         // chains stepped by the caller (b2n_ns_rwalk_step)
+    if (!stepped && (c->model_id < 0 || c->model_id >= (int)ctx->models.size())) return B2N_ERR_ARG;
+    if (stepped && (c->sampler != 0 || c->unit_cube_phase))
+        return b2n_fail(ctx, B2N_ERR_ARG, "b2n_ns_create: a run without an in-kernel model has stepped rwalk chains and no unit-cube phase");
+    const int n = stepped ? c->ndim : ctx->models[c->model_id].ndim;
     if (c->ndim != n || c->nlive < 2 || c->batch < 1 || c->batch >= c->nlive || c->steps < 1 || c->sampler < 0 ||
         c->sampler > 3 || c->ncdim < 1 || c->ncdim > n)
         return b2n_fail(ctx, B2N_ERR_ARG, "b2n_ns_create: need 1 <= batch < nlive, steps >= 1, sampler in {0,1,2,3}, ndim == model ndim");
@@ -787,25 +824,10 @@ int b2n_ns_run(b2n_ctx* ctx, int32_t max_rounds, int32_t check_every, b2n_ns_sta
     NsDev& d = ns->d;
     B2N_CUDA(ctx, cudaSetDevice(ctx->device));
     if (ctx->peer.total > 0) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "b2n_ns_run: gather mode must be off");
-    if (ns->phase == 0) {            // unit-cube rounds: no bound yet
-        d.Kell = 1;
-        d.ctrs = d.ams = d.logvols = nullptr;
-    } else {
-        if (ctx->bK < 1 || ctx->bn != d.nc) return b2n_fail(ctx, B2N_ERR_ARG, "resident bound missing or of wrong dimension (b2n_bound_set)");
-        if (!ctx->b_ctrs.p || !ctx->b_ams.p || !ctx->b_logvols.p || ctx->h_logvols.empty())
-            return b2n_fail(ctx, B2N_ERR_ARG, "b2n_ns_run needs the full resident bound (ctrs, ams, logvols)");
-        d.Kell = ctx->bK;
-        d.ctrs = ctx->b_ctrs.as<double>(); d.ams = ctx->b_ams.as<double>(); d.logvols = ctx->b_logvols.as<double>();
-    }
-    d.strict = ns->cfg.strict_contains;
-    if ((size_t)d.K / 1 + (size_t)d.Kell + 8 > (size_t)d.K + (size_t)d.N + 8)
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "too many ellipsoids for the round worklist");
-    B2N_TRY(ns_chain_call(ctx, ns, true));               // chains per CTA the chain kernel plans for
-    d.cpc = ctx->dyn.cpc;
-    const size_t smem = std::max(ns_propose_smem(d), ns_commit_smem(d));
-    if (smem + 2048 > (size_t)ctx->max_smem_optin)
-        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "nlive / batch too large for the one-CTA kernels of b2n_ns_run");
-    B2N_TRY(b2n_func_smem(ctx, (const void*)(ns_step_kernel), (size_t)(smem)));
+    if (ns->cfg.model_id < 0)
+        return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "b2n_ns_run: the run has no in-kernel model (its chains are stepped: b2n_ns_step / b2n_ns_rwalk_step)");
+    size_t smem;
+    B2N_TRY(ns_prepare(ctx, ns, &smem));
     if (check_every < 1) check_every = max_rounds > 0 ? max_rounds : 1;
     int left = max_rounds;
     b2n_ns_status st;
@@ -866,6 +888,41 @@ int b2n_ns_run(b2n_ctx* ctx, int32_t max_rounds, int32_t check_every, b2n_ns_sta
         return st.error;
     }
     return B2N_OK;
+}
+
+int b2n_ns_step(b2n_ctx* ctx, int32_t mode) {
+    if (!ctx || !ctx->ns || !ctx->ns->active || (mode != 1 && mode != 3)) return B2N_ERR_ARG;
+    b2n_ns* ns = ctx->ns;
+    if (ns->cfg.model_id >= 0) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "b2n_ns_step drives runs with stepped chains; b2n_ns_run the others");
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    size_t smem;
+    B2N_TRY(ns_prepare(ctx, ns, &smem));
+    ns_step_kernel<<<1, ns->d.threads, smem, ctx->stream>>>(ns->d, mode);
+    B2N_LAUNCH_CHECK(ctx);
+    return B2N_OK;
+}
+
+int b2n_ns_rwalk_step(b2n_ctx* ctx, int32_t step, b2n_rwalk_state* st) {
+    if (!ctx || !ctx->ns || !ctx->ns->active) return B2N_ERR_ARG;
+    b2n_ns* ns = ctx->ns;
+    const NsDev& d = ns->d;
+    if (ns->cfg.model_id >= 0) return b2n_fail(ctx, B2N_ERR_UNSUPPORTED, "b2n_ns_rwalk_step: the run's chains run in-kernel (b2n_ns_run)");
+    if (step == 0 && (!st || !st->u_start)) return b2n_fail(ctx, B2N_ERR_ARG, "b2n_ns_rwalk_step: step 0 needs u_start (the round's start rows)");
+    if (ctx->bK < 1 || ctx->bn != d.nc) return b2n_fail(ctx, B2N_ERR_ARG, "resident bound missing or of wrong dimension (b2n_bound_set)");
+    RwalkStepParams p;
+    memset(&p, 0, sizeof(p));
+    B2N_TRY(b2n_rwalk_step_bind(ctx, ns->cfg.steps, step, st, p));
+    B2N_CUDA(ctx, cudaSetDevice(ctx->device));
+    int cpc, warps;
+    size_t smem;
+    B2N_TRY(b2n_rwalk_step_plan(ctx, d.K, d.n, &cpc, &warps, &smem));
+    p.n = d.n; p.nc = d.nc; p.u0 = d.u0;
+    p.order = d.order; p.cta = d.cta;
+    p.axesT = ctx->b_axesT.as<double>();
+    p.seed = d.seed; p.dyn = d.dyn;
+    p.u = d.o_u; p.v = d.o_v; p.logl = d.o_logl; p.nacc = d.o_i0; p.nrej = d.o_i1; p.ncall = d.o_ncall;
+    const unsigned grid = d.cpc > 0 ? (unsigned)(d.K / d.cpc + d.Kell) : 1u;     // ns_chain_call's bound
+    return b2n_rwalk_step_launch(ctx, p, grid, warps, smem);
 }
 
 __global__ void ns_set_counters_kernel(NsScalars* sc, long long rounds, long long ncall_last_update, int doubling) {

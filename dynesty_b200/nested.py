@@ -25,6 +25,7 @@ import numpy as np
 
 from . import bounding as B
 from . import samplers as S
+from .torchmodel import TorchModel
 
 LOWL = -1e300
 
@@ -89,6 +90,9 @@ class NestedSampler:
     the ranks and all-gathered (NCCL), every rank keeps the identical host state.
     `live_points`: (u, v, logl), or the reference's (u, v, logl, blobs); the blobs are not read, because the blob of
     every saved sample is computed from its v at the end of the run.
+    `model` may also be a ``TorchModel`` (batched PyTorch callables): the rwalk chains are then stepped, the live
+    points drawn on the host and the phase before the first bound runs in the host loop.
+    `device_init`: the default of ``run_nested(device_init=)``.
     `blob`: save the model's blob with every sample, as ``results['blob']`` (nsamples x model.nblob).  It needs a
     model with blobs (``DeviceModel.from_cuda(..., nblob=k)``).  The chains do not carry it: the blob is a
     deterministic function of v, evaluated once per saved sample by one launch at the end of the run.
@@ -97,7 +101,20 @@ class NestedSampler:
     def __init__(self, model, nlive=500, bound='multi', sample='auto', ncdim=None, walks=None, slices=None,
                  facc=0.5, enlarge=None, bootstrap=None, update_interval=None, first_update=None,
                  queue_size=None, periodic=None, reflective=None, seed=56432, ctx=None, comm=None, live_points=None,
-                 live_init='device', blob=False):
+                 live_init='device', blob=False, device_init=True):
+        self.torch_model = isinstance(model, TorchModel)
+        if self.torch_model:
+            # the likelihood runs between the launches of the stepped random walk (dynesty_b200/torchmodel.py)
+            if isinstance(sample, str) and sample in ('unif', 'slice', 'rslice'):
+                raise NotImplementedError("sample=%r with a TorchModel: only the random walk ('rwalk') is stepped"
+                                          % sample)
+            if blob:
+                raise ValueError('blob=True is not available for a TorchModel')
+            if comm is not None:
+                raise ValueError("comm= is not available for a TorchModel: its chains run on one GPU")
+            if sample == 'auto':
+                sample = 'rwalk'
+            live_init, device_init = 'host', False
         if blob and getattr(model, 'nblob', 0) < 1:
             raise ValueError('blob=True needs a model with blobs: DeviceModel.from_cuda(..., nblob=k) with a source '
                              'that defines b2n_user_blob')
@@ -110,6 +127,7 @@ class NestedSampler:
         self.seed = int(seed)
         self.ctx = ctx
         self.comm = comm
+        self.device_init = bool(device_init)
         # -- inner sampler (dynesty.py:126-166)
         if sample == 'auto':
             sample = 'unif' if n < 10 else ('rwalk' if n <= 20 else 'rslice')
@@ -526,7 +544,8 @@ class NestedSampler:
                     due = self.ncall_at_last_update + self.bound_update_interval - self.ncall
                     want = int(min(4096, max(1, math.ceil(due / per_round))))
                 t0 = time.perf_counter()
-                st = ops.ns_run(want, 0, ctx=self.ctx)
+                st = ops.ns_run_stepped(self.model, want, ctx=self.ctx) if getattr(self, 'torch_model', False) else \
+                    ops.ns_run(want, 0, ctx=self.ctx)
                 tm['rounds_s'] += time.perf_counter() - t0
                 rounds, self.ncall = st['rounds'], st['ncall']
                 self.eff = 100. * (it0 + st['it']) / max(self.ncall, 1)
@@ -591,7 +610,7 @@ class NestedSampler:
 
     # ------------------------------------------------------------------ main loop
     def run_nested(self, dlogz=None, maxiter=None, maxcall=None, add_live=True, loop='host', batch=None,
-                   checkpoint_file=None, checkpoint_every=60., resume=False, on_checkpoint=None, device_init=True,
+                   checkpoint_file=None, checkpoint_every=60., resume=False, on_checkpoint=None, device_init=None,
                    keep_samples=True, logl_max=None, strands=False):
         """sampler.py:1214-1356 / 1040-1212 (no plateau mode: continuous likelihoods).
 
@@ -610,11 +629,18 @@ class NestedSampler:
                         device (results.samples / samples_u are then empty; logz, logzerr, logl, logvol, logwt and the
                         call counts are complete): for ensembles that only want evidences.  Not with blob=True.
         device_init   : False = the phase before the first bound runs in the host loop (queue of prior draws
-                        evaluated on the GPU) and the device takes over when the first bound exists.
+                        evaluated on the GPU) and the device takes over when the first bound exists.  None: the
+                        sampler's ``device_init`` (always False for a TorchModel).
         strands       : True = record every sample's strand (the reference's samples_id / samples_it): the results
                         then carry samples_id, the live slot the point occupied, and samples_it, the number of dead
                         points of the run recorded before it entered the live set; resample_run and unravel_run
                         (dynesty_b200.utils) need them."""
+        if getattr(self, 'torch_model', False):
+            if checkpoint_file is not None:
+                raise ValueError('checkpoint_file= is not available for a TorchModel: its callables need not pickle')
+            device_init = False
+        elif device_init is None:
+            device_init = getattr(self, 'device_init', True)
         if resume:
             return self._resume(checkpoint_file, checkpoint_every)
         if loop not in ('host', 'device'):

@@ -364,6 +364,90 @@ def rwalk_batch(model, u0, loglstar, scale, walks, seed, chain0=0, ncdim=None, e
     return o
 
 
+# ---- stepped random walk of a TorchModel (include/b200nest.h, b2n_rwalk_step / b2n_ns_rwalk_step) ---------------
+class _torch_stream:
+    """Context manager: the library works on torch's current stream of `device`, in device-pointer mode, and the
+    previous stream and pointer mode come back however the block ends.  (torch's default stream, handle 0, is the
+    legacy default stream: passed as cudaStreamLegacy, 1, since a NULL stream means the context's own.)"""
+
+    def __init__(self, ctx, device):
+        import torch
+        self.ctx = ctx
+        self.stream = torch.cuda.current_stream(device).cuda_stream or 1
+
+    def __enter__(self):
+        c = self.ctx
+        self.prev_stream, self.prev_mode = c.stream, c.mode
+        if self.stream != c.stream:
+            c.set_stream(self.stream)
+        c.set_pointer_mode(_lib.PTR_DEVICE)
+
+    def __exit__(self, *exc):
+        c = self.ctx
+        try:
+            c.set_pointer_mode(self.prev_mode)
+        finally:
+            if c.stream != self.prev_stream:
+                c.set_stream(self.prev_stream)
+        return False
+
+
+def _step_state(Q, n, device, dimflags, worklist):
+    """A b2n_rwalk_state over fresh device buffers for Q chains; returns (state, buffers)."""
+    import torch
+    b = dict(u_prop=torch.full((Q, n), 0.5, dtype=torch.float64, device=device),
+             tick=torch.zeros(Q, dtype=torch.int32, device=device),
+             in_cube=torch.zeros(Q, dtype=torch.int32, device=device))
+    if dimflags is not None:
+        b['dimflags'] = torch.as_tensor(np.asarray(dimflags, dtype=np.int32), device=device)
+    if worklist:
+        b['order'] = torch.empty(Q, dtype=torch.int32, device=device)
+        b['cta'] = torch.empty(3 * Q, dtype=torch.int32, device=device)
+    else:
+        b['u_start'] = torch.full((Q, n), 0.5, dtype=torch.float64, device=device)
+    st = _lib.RwalkState()
+    for k, t in b.items():
+        setattr(st, k, t.data_ptr())
+    return st, b
+
+
+def _step_through(model, walks, launch, st, u_start, u_prop):
+    """walks + 1 stepped launches with the model's calls between them, all enqueued on the current stream: launch(s)
+    enqueues step s; the start rows u_start are evaluated after step 0 (which writes them in a device round), the
+    proposals u_prop after every step but the last."""
+    for s in range(walks + 1):
+        launch(s)
+        if s == 0:
+            v_start, l_start = model._eval(u_start)     # (kept alive until the last launch has been enqueued)
+            st.v_start, st.logl_start = v_start.data_ptr(), l_start.data_ptr()
+        if s < walks:
+            v_prop, l_prop = model._eval(u_prop)
+            st.v_prop, st.logl_prop = v_prop.data_ptr(), l_prop.data_ptr()
+
+
+def rwalk_stepped(model, u0, loglstar, scale, walks, seed, chain0=0, ell=None, dimflags=None, ncdim=None, ctx=None):
+    """rwalk_batch for a TorchModel: the same chains (same random streams, same proposals) with the likelihood
+    evaluated by the model's torch callables between walks + 1 launches of the stepped kernel, on torch's current
+    stream and with no host synchronisation until the outputs are read.  u0: numpy or a CUDA tensor (Q, ndim).
+    Returns rwalk_batch's dict of numpy arrays."""
+    import torch
+    ctx = _ctx(ctx)
+    dev = model.device(ctx)
+    u0 = torch.as_tensor(u0, dtype=torch.float64, device=dev).contiguous()
+    a, keep, Q, n = _chain_args(-1, u0, ncdim, loglstar, scale, seed, chain0, ell, None)
+    st, bufs = _step_state(Q, n, dev, dimflags, worklist=True)
+    o = dict(u=torch.empty((Q, n), dtype=torch.float64, device=dev), v=torch.empty((Q, n), dtype=torch.float64, device=dev),
+             logl=torch.empty(Q, dtype=torch.float64, device=dev))
+    for k in _lib.CHAIN_OUTPUTS['rwalk'][:3]:
+        o[k] = torch.empty(Q, dtype=torch.int32, device=dev)
+    args = _chain_ptrs(o, 'rwalk')
+    with _torch_stream(ctx, dev):
+        _step_through(model, int(walks),
+                      lambda s: ctx.check(ctx.lib.b2n_rwalk_step(ctx.h, C.byref(a), int(walks), s, C.byref(st), *args)),
+                      st, u0, bufs['u_prop'])
+        return {k: t.cpu().numpy() for k, t in o.items()}
+
+
 def _slice_batch(fn, model, u0, loglstar, scale, slices, seed, chain0, doubling, ell, ctx, peer=None):
     ctx = _ctx(ctx)
     a, keep, Q, n = _chain_args(model, u0, None, loglstar, scale, seed, chain0, ell, None)
@@ -421,6 +505,7 @@ def ns_create(model, nlive, ndim, batch, sampler, steps, seed, chain0=0, ncdim=N
               dead_capacity=None, ctx=None, unit_cube_phase=False, first_min_ncall=0, first_min_eff=100., it0=0,
               logl_max=None):
     """Allocate the device state of a batched-replacement run (sampler: 0 rwalk, 1 rslice, 2 slice, 3 unif).
+    model = -1: no in-kernel model, the rwalk chains are stepped with a TorchModel (ns_run_stepped).
     unit_cube_phase: start with rounds that draw from the prior until the first bound is due
     (need_bound = 4 once ncall >= first_min_ncall and 100 (it0 + it) / ncall < first_min_eff)."""
     ctx = _ctx(ctx)
@@ -439,7 +524,10 @@ def ns_create(model, nlive, ndim, batch, sampler, steps, seed, chain0=0, ncdim=N
         float(first_min_eff), int(it0)
     c.use_logl_max, c.logl_max = (0, 0.0) if logl_max is None else (1, float(logl_max))
     cap = int(dead_capacity) if dead_capacity is not None else 64 * int(nlive)
+    ctx.ns_stepped = None
     ctx.check(ctx.lib.b2n_ns_create(ctx.h, C.byref(c), cap))
+    if int(model) == -1:         # no in-kernel model: the chains are stepped (ns_run_stepped)
+        ctx.ns_stepped = (int(batch), int(ndim), int(steps), dimflags)
 
 
 def ns_set_state(live_u, live_v, live_logl, logvol, logz, loglstar, ncall, scale, ctx=None):
@@ -460,6 +548,31 @@ def ns_run(max_rounds, check_every=0, ctx=None):
     st = _lib.NsStatus()
     ctx.check(ctx.lib.b2n_ns_run(ctx.h, int(max_rounds), int(check_every), C.byref(st)))
     return _ns_status(st)
+
+
+def ns_run_stepped(model, max_rounds, ctx=None):
+    """ns_run for a run created with a TorchModel (ns_create(model_id=-1)): enqueue max_rounds rounds, each
+    b2n_ns_step(3) then walks + 1 x (b2n_ns_rwalk_step, torch call), and the closing commit b2n_ns_step(1), on torch's
+    current stream; read the status once at the end.  Returns ns_run's status dict."""
+    ctx = _ctx(ctx)
+    if ctx.ns_stepped is None:
+        raise ValueError("ns_run_stepped needs a run created with a TorchModel (ns_create(model_id=-1))")
+    K, n, walks, dimflags = ctx.ns_stepped
+    dev = model.device(ctx)
+    st, bufs = _step_state(K, n, dev, dimflags, worklist=False)
+    with _torch_stream(ctx, dev):
+        for _ in range(int(max_rounds)):
+            ctx.check(ctx.lib.b2n_ns_step(ctx.h, 3))
+            _step_through(model, walks, lambda s: ctx.check(ctx.lib.b2n_ns_rwalk_step(ctx.h, s, C.byref(st))), st,
+                          bufs['u_start'], bufs['u_prop'])
+        if max_rounds > 0:
+            ctx.check(ctx.lib.b2n_ns_step(ctx.h, 1))
+        s = ns_status(ctx)
+    if s['error']:
+        raise _lib._EXC.get(s['error'], RuntimeError)(
+            "device rounds stopped with status %d after round %d (it %d, ncall %d)"
+            % (s['error'], s['rounds'], s['it'], s['ncall']))
+    return s
 
 
 def ns_status(ctx=None):

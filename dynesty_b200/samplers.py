@@ -20,6 +20,7 @@ import numpy as np
 from . import ops, _lib
 from ._compat import InternalSamplerBase, SamplerReturn
 from .bounding import TaggedAxes
+from .torchmodel import TorchModel
 
 __all__ = ['B200RWalkSampler', 'B200RSliceSampler', 'B200SliceSampler', 'B200UniformSampler']
 
@@ -130,6 +131,11 @@ class B200RWalkSampler(_B200Sampler):
 
     def run_batch(self, loglstar, points, ell, seed, chain0=0, peer=None):
         walks = self.sampler_kwargs['walks']
+        if isinstance(self.model, TorchModel):       # the likelihood runs between the launches of the stepped walk
+            if peer is not None:
+                raise NotImplementedError("a TorchModel's chains run on one GPU")
+            return ops.rwalk_stepped(self.model, points, loglstar, self.scale, walks, seed, chain0=chain0, ell=ell,
+                                     dimflags=self._flags(), ncdim=self.ncdim or self.model.ndim, ctx=self._ctx)
         return ops.rwalk_batch(self.model.model_id(self._ctx), points, loglstar, self.scale, walks, seed,
                                chain0=chain0, ncdim=self.ncdim or self.model.ndim, ell=ell,
                                dimflags=self._flags(), ctx=self._ctx, peer=peer)

@@ -537,6 +537,41 @@ int b2n_rwalk_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t walks,
                     double* u, double* v, double* logl,
                     int32_t* n_accept, int32_t* n_reject, int32_t* ncall);
 
+/* ---- stepped random walk: the walk of b2n_rwalk_batch, one launch per step, for a likelihood that runs OUTSIDE the
+ * library between the launches (a batched PyTorch function on the same stream, dynesty_b200.TorchModel).
+ * A fill of Q chains is walks + 1 calls, step = 0 .. walks, each enqueuing one launch and no synchronisation:
+ *   step 0        chain q starts at u0[q] (u written, u_start[q] too when given) and proposes step 0
+ *   step s        accepts step s - 1 -- inside the cube and logl_prop[q] > loglstar: u, v, logl <- the proposal and
+ *                 n_accept + 1, else n_reject + 1 (a NaN logl_prop is rejected) -- then proposes step s
+ *   step walks    accepts step walks - 1; a chain that never accepted gets v_start / logl_start; ncall = walks
+ * A proposal writes u_prop[q] and in_cube[q]; an out-of-cube proposal's row of u_prop is the chain's current u, so
+ * that the caller only ever evaluates points of the cube.  Between step s and s + 1 the caller puts the prior
+ * transform of u_prop in v_prop and its log-likelihood in logl_prop; before step `walks` the same for the start rows
+ * in v_start / logl_start.  Chain q draws from the B2N stream (seed, chain0 + q) exactly as in b2n_rwalk_batch, so
+ * a likelihood that returns the bits the in-kernel one does gives bit-identical chains.  Every pointer is a device
+ * pointer, and the fields are re-read at every call (the caller may point v_prop at a new buffer each step). */
+typedef struct {
+    double*         u_prop;      /* Q x ndim, out                                                       */
+    const double*   v_prop;      /* Q x ndim, in (steps >= 1): prior transform of u_prop                */
+    const double*   logl_prop;   /* Q, in (steps >= 1)                                                  */
+    double*         u_start;     /* Q x ndim, out at step 0 (a copy of the start rows), may be NULL     */
+    const double*   v_start;     /* Q x ndim, in (step walks): prior transform of the start rows        */
+    const double*   logl_start;  /* Q, in (step walks)                                                  */
+    uint32_t*       tick;        /* Q: next draw event of every chain                                   */
+    int32_t*        in_cube;     /* Q: the last proposal lies inside the cube                           */
+    const uint32_t* dimflags;    /* ndim B2N_DIM_* flags (device, uint32) or NULL; b2n_chain_args.dimflags is not read */
+    int32_t*        order;       /* Q, written at step 0 (b2n_rwalk_step): the chains grouped by ellipsoid */
+    int32_t*        cta;         /* 3 x Q, written at step 0 (b2n_rwalk_step): (first, count, ellipsoid) per CTA */
+    int32_t         ncta;        /* out at step 0 (b2n_rwalk_step), in at later steps                   */
+    int32_t         reserved;
+} b2n_rwalk_state;
+
+/* One step of a host fill: a = the fill's chains as for b2n_rwalk_batch (u0 a device pointer; ell read at step 0
+ * only), outputs as b2n_rwalk_batch's, which also hold the chains' state between the calls.  Needs
+ * B2N_PTR_DEVICE, the resident bound, no gather mode and no pending b2n_set_start_rows. */
+int b2n_rwalk_step(b2n_ctx* ctx, const b2n_chain_args* a, int32_t walks, int32_t step, b2n_rwalk_state* st,
+                   double* u, double* v, double* logl, int32_t* n_accept, int32_t* n_reject, int32_t* ncall);
+
 /* RSliceSampler.sample (internal_samplers.py:745-855) / SliceSampler.sample
  * (:593-709) -> generic_slice_step (:1075-1206).  flags[q]: B2N_WARN_DOUBLING if
  * the chain switched to doubling; status B2N_ERR_SLICE_FAIL if any chain's
@@ -697,6 +732,18 @@ int b2n_ns_set_state(b2n_ctx* ctx, const double* live_u, const double* live_v, c
  * the end); synchronises; returns the status (and the sampler error status, e.g.
  * B2N_ERR_SLICE_FAIL, if a chain failed). */
 int b2n_ns_run(b2n_ctx* ctx, int32_t max_rounds, int32_t check_every, b2n_ns_status* status);
+/* Rounds whose chains are STEPPED (b2n_rwalk_step's walk, likelihood outside the library).  b2n_ns_create takes
+ * model_id = -1 ("no in-kernel model") for such a run: sampler 0 (rwalk), unit_cube_phase 0, ndim from the config;
+ * b2n_ns_run refuses it with B2N_ERR_UNSUPPORTED.  The caller enqueues, with no synchronisation in between,
+ *   b2n_ns_step(3) | b2n_ns_rwalk_step(0) .. b2n_ns_rwalk_step(steps)   per round, then b2n_ns_step(1),
+ * with its likelihood between the stepped launches as for b2n_rwalk_step (start rows: st->u_start, which step 0
+ * must be given here), and reads the flags with b2n_ns_status_get.
+ * b2n_ns_step: one launch of the round kernel; mode 3 = commit the pending round and propose the next, 1 = the
+ * closing commit.  b2n_ns_rwalk_step: one stepped launch bound to the current round -- threshold, scale, chain ids,
+ * worklist and skip from the round's device state, start rows and outputs the round's own buffers; the order / cta /
+ * ncta fields of st are not used.  A round skipped on the device (a stop flag) makes its launches return at once. */
+int b2n_ns_step(b2n_ctx* ctx, int32_t mode);
+int b2n_ns_rwalk_step(b2n_ctx* ctx, int32_t step, b2n_rwalk_state* st);
 int b2n_ns_status_get(b2n_ctx* ctx, b2n_ns_status* status);
 /* restore the counters a snapshot of a run carries besides b2n_ns_set_state's arguments (utils.py:2321-2355
  * save / restore of the reference pickles the whole sampler; here: live set + scalars + these): the round
