@@ -5,6 +5,7 @@
 #include "b2n_chain.cuh"
 
 #define B2N_MAX_EXPAND 4000000      // hard stop against a runaway stepping-out loop
+#define B2N_EXPAND_SAT 0x7fffffff   // a chain's n_expand saturates here instead of wrapping
 
 struct SliceParams {
     B2nModel m;
@@ -66,7 +67,9 @@ __device__ bool doubling_accept(EVAL& F, double x1, double loglstar, double L, d
 }
 
 // one generic_slice_step along b2n_sm[odir..] (already scaled, not yet length-capped).  On
-// success the new point is left in b2n_sm[F.oun..] and its logl returned.
+// success the new point is left in b2n_sm[F.oun..] and its logl returned.  D doublings count 2^D - 1 expansions
+// (a tiny scale takes 40 or more).  The reference counts in Python ints; here the step's count and n_expand, the
+// chain's total, saturate at B2N_EXPAND_SAT (INT32_MAX) instead of wrapping.
 template <class EVAL>
 __device__ double slice_step(EVAL& F, ChainRng& g, double loglstar, bool doubling, int& n_expand, int& n_contract,
                              bool& expansion_warning, int& err) {
@@ -97,17 +100,17 @@ __device__ double slice_step(EVAL& F, ChainRng& g, double loglstar, bool doublin
         }
         if (nexp > 1000) expansion_warning = true;              // :1142-1145
     } else {
-        int K = 1;                                              // :1149-1163
+        int D = 0;                                              // :1149-1163 (n_expand += K, K *= 2)
         while (fl > loglstar || fr > loglstar) {
             const double V = rng_uniform(g);
             if (V < 0.5) { xl -= (xr - xl); fl = F(xl); }
             else { xr += (xr - xl); fr = F(xr); }
-            nexp += K;
-            if (K < (1 << 28)) K *= 2;
+            D++;
         }
+        nexp = D < 31 ? (1 << D) - 1 : B2N_EXPAND_SAT;
         L = xl; R = xr; fL = fl; fR = fr;
     }
-    n_expand += nexp;
+    n_expand = (int)min((long long)n_expand + nexp, (long long)B2N_EXPAND_SAT);
     double lp = -INFINITY;
     for (int it = 0; !err; it++) {                              // :1168-1203
         const double xp = xl + rng_uniform(g) * (xr - xl);

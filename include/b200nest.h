@@ -575,7 +575,9 @@ int b2n_rwalk_step(b2n_ctx* ctx, const b2n_chain_args* a, int32_t walks, int32_t
 /* RSliceSampler.sample (internal_samplers.py:745-855) / SliceSampler.sample
  * (:593-709) -> generic_slice_step (:1075-1206).  flags[q]: B2N_WARN_DOUBLING if
  * the chain switched to doubling; status B2N_ERR_SLICE_FAIL if any chain's
- * interval collapsed. */
+ * interval collapsed or stepped out more than 4e6 times.  n_expand[q] saturates at
+ * INT32_MAX (a step with D doublings counts 2^D - 1, and a tiny scale takes 31 or
+ * more), where the reference's count keeps growing. */
 int b2n_rslice_batch(b2n_ctx* ctx, const b2n_chain_args* a, int32_t slices,
                      int32_t doubling, double* u, double* v, double* logl,
                      int32_t* n_expand, int32_t* n_contract, int32_t* ncall,

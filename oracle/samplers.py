@@ -111,9 +111,13 @@ def _doubling_accept(x1, F, loglstar, L, R, fL, fR):
     return True
 
 
-def slice_step(u, direction, loglstar, model, stream, doubling):
+def slice_step(u, direction, loglstar, model, stream, doubling, stats=None):
     """generic_slice_step (:1075-1206).  Returns
-    (u_new, logl_new, nc, n_expand, n_contract, expansion_warning)."""
+    (u_new, logl_new, nc, n_expand, n_contract, expansion_warning).
+
+    `stats`, if a dict, receives counts of the branches the step took (they change nothing it returns):
+    'capped' (1 if the direction was shortened to sqrt(n)/2), 'doublings' (intervals doubled) and
+    'doubling_rejects' (proposals inside the slice that _doubling_accept refused)."""
     n = len(u)
     n_expand = n_contract = 0
     rand0 = stream.uniform()                                      # :1099
@@ -125,6 +129,7 @@ def slice_step(u, direction, loglstar, model, stream, doubling):
     fl, fr = F(xl)[1], F(xr)[1]
     warn = False
     L = R = fL = fR = None
+    ndbl = nrej = 0
     if not doubling:
         while fl > loglstar:                                      # :1134-1141
             xl -= 1
@@ -146,64 +151,89 @@ def slice_step(u, direction, loglstar, model, stream, doubling):
                 fr = F(xr)[1]
             n_expand += K
             K *= 2
+            ndbl += 1
         L, R, fL, fR = xl, xr, fl, fr
     while True:                                                   # :1168-1203
         xp = xl + stream.uniform() * (xr - xl)
         up, lp = F(xp)
         n_contract += 1
-        if lp > loglstar and (not doubling or
-                              _doubling_accept(xp, F, loglstar, L, R, fL, fR)):
-            break
+        if lp > loglstar:
+            if not doubling or _doubling_accept(xp, F, loglstar, L, R, fL, fR):
+                break
+            nrej += 1
         if xp < 0:
             xl = xp
         elif xp > 0:
             xr = xp
         else:
             raise RuntimeError("Slice sampler has failed to find a valid point.")
+    if stats is not None:
+        stats.update(capped=int(dirlen > maxlen), doublings=ndbl, doubling_rejects=nrej)
     return up, lp, F.nc, n_expand, n_contract, warn
+
+
+def _stats_init():
+    """Per-chain branch counters of rslice_chain / slice_chain (see slice_step): doublings per step, steps with a
+    capped direction, _doubling_accept rejections, and the slice / step index at which the expansion warning fired."""
+    return dict(doublings=[], n_capped=0, n_doubling_rejects=0, warn_slice=None, warn_step=None)
+
+
+def _stats_add(st, s, sl, step, w, doubling):
+    st['doublings'].append(s['doublings'])
+    st['n_capped'] += s['capped']
+    st['n_doubling_rejects'] += s['doubling_rejects']
+    if w and not doubling:
+        st['warn_slice'], st['warn_step'] = sl, step
 
 
 def rslice_chain(u0, loglstar, axes, scale, model, stream, slices,
                  doubling=False):
-    """RSliceSampler.sample (:745-855)."""
+    """RSliceSampler.sample (:745-855).  The returned dict also carries the branch counters of _stats_init."""
     u = np.array(u0, dtype=float)
     n = u.shape[0]
     nc = nexp = ncon = 0
     warned = False
     logl = None
-    for _ in range(slices):
+    st = _stats_init()
+    for sl in range(slices):
         z = stream.normals(n)                                     # :820-821
         z = z / math.sqrt(float(np.dot(z, z)))
         direction = np.dot(axes, z) * scale                       # :824
+        s = {}
         u, logl, c, e, k, w = slice_step(u, direction, loglstar, model, stream,
-                                         doubling)
+                                         doubling, s)
         nc, nexp, ncon = nc + c, nexp + e, ncon + k
+        _stats_add(st, s, sl, sl, w, doubling)
         if w and not doubling:                                    # :836-838
             doubling = warned = True
     return dict(u=u, v=model.prior_transform(u), logl=logl, ncall=nc,
                 n_expand=nexp, n_contract=ncon, expansion_warning_set=warned,
-                ticks=stream.tick)
+                ticks=stream.tick, **st)
 
 
 def slice_chain(u0, loglstar, axes, scale, model, stream, slices,
                 doubling=False):
-    """SliceSampler.sample (:593-709): principal-axis Gibbs-like slices."""
+    """SliceSampler.sample (:593-709): principal-axis Gibbs-like slices.  The returned dict also carries the branch
+    counters of _stats_init (steps are counted over all slices: slice sl, axis j is step sl * n + j)."""
     u = np.array(u0, dtype=float)
     n = u.shape[0]
     ax = scale * axes.T                                           # :665
     nc = nexp = ncon = 0
     warned = False
     logl = None
-    for _ in range(slices):
-        for i in stream.permutation(n):                           # :673-677
+    st = _stats_init()
+    for sl in range(slices):
+        for j, i in enumerate(stream.permutation(n)):             # :673-677
+            s = {}
             u, logl, c, e, k, w = slice_step(u, ax[i], loglstar, model, stream,
-                                             doubling)
+                                             doubling, s)
             nc, nexp, ncon = nc + c, nexp + e, ncon + k
+            _stats_add(st, s, sl, sl * n + j, w, doubling)
             if w and not doubling:
                 doubling = warned = True
     return dict(u=u, v=model.prior_transform(u), logl=logl, ncall=nc,
                 n_expand=nexp, n_contract=ncon, expansion_warning_set=warned,
-                ticks=stream.tick)
+                ticks=stream.tick, **st)
 
 
 def unitcube_chain(loglstar, model, stream, ndim, max_tries=10**7):
