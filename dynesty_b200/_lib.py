@@ -156,6 +156,11 @@ SYMBOLS = {
     'b2n_resample_runs': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _P, _P, _P, _P]),
     'b2n_resample_posterior': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _P, _I, _P, _I,
                                          _P, _P, _P, _P, _P, _P, _P]),
+    'b2n_resample_equal': (C.c_int, [_P, _P, _L, _I, _L, _U64, _U64, _P, _I, _P, _P, _P, _P]),
+    'b2n_jitter_equal': (C.c_int, [_P, _P, _P, _L, _P, _D, _I, _I, _U64, _U64, _L, _P, _I, _P, _P, _P, _P, _P, _P,
+                                   _P, _P]),
+    'b2n_resample_equal_runs': (C.c_int, [_P, _P, _P, _L, _I, _P, _P, _P, _P, _P, _D, _I, _U64, _U64, _L, _P, _I,
+                                          _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_merge_runs': (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2n_compute_integrals': (C.c_int, [_P, _P, _P, _P, _L, _P, _P, _P, _P, _P]),
     'b2n_set_reweight': (C.c_int, [_P, _P, _L]),

@@ -344,6 +344,18 @@ struct B2nOutStage {
         return B2N_OK;
     }
 };
+// Bump allocation in one buffer (256-byte aligned pieces); a first pass with base == NULL measures it.
+struct Bump {
+    char* base;
+    size_t off = 0;
+    template <class T> T* take(size_t count) {
+        off = (off + 255) / 256 * 256;
+        T* p = (T*)(base ? base + off : nullptr);
+        off += count * sizeof(T);
+        return p;
+    }
+};
+
 // The log-reweight of b2n_set_reweight / b2n_compute_integrals: in host-pointer mode NaN and +inf are refused (device
 // arrays are the caller's to check).
 static inline int b2n_reweight_check(b2n_ctx* ctx, const double* lrw, int64_t N) {

@@ -311,18 +311,6 @@ __global__ void __launch_bounds__(32) quant_lookup_kernel(QArgs A) {
         if (Cp <= A.q[t]) out[t] = xp;
 }
 
-// Bump allocation in one buffer (256-byte aligned pieces); a first pass with base == NULL measures it.
-struct Bump {
-    char* base;
-    size_t off = 0;
-    template <class T> T* take(size_t count) {
-        off = (off + 255) / 256 * 256;
-        T* p = (T*)(base ? base + off : nullptr);
-        off += count * sizeof(T);
-        return p;
-    }
-};
-
 struct PostJob {
     int64_t N;
     int n, R, nq;

@@ -50,6 +50,12 @@ class Results(dict):
         wt = np.exp(self['logwt'] - self['logz'][-1])
         return wt / wt.sum()
 
+    def samples_equal(self, rstate=None, seed=None):
+        """The equally weighted samples in random order (utils.py:895-903): resample_equal of the samples under
+        importance_weights(); see dynesty_b200.utils.resample_equal for rstate / seed."""
+        from .utils import resample_equal
+        return resample_equal(self['samples'], self.importance_weights(), rstate=rstate, seed=seed)
+
     def posterior_moments(self):
         w = np.exp(self['logwt'] - self['logz'][-1])
         w /= w.sum()

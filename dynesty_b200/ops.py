@@ -877,6 +877,99 @@ def resample_posterior(logl, strand, base, piece_ptr, piece_strand, end, x, R, s
     return o
 
 
+# ---- equal-weight draws (include/b200nest.h, b2n_resample_equal / b2n_jitter_equal / b2n_resample_equal_runs) ------
+EQUAL_CHAIN0 = 1 << 62          # B2N_EQUAL_CHAIN0: the draws of realisation r use the stream (seed, this + chain0 + r)
+
+
+def _equal_outputs(R, N, M, x, counts):
+    """The outputs of an equal-weight call: idx (R x M), wsum (R), counts (R x N) with counts, x (R x M x k) with x."""
+    o = dict(idx=np.empty((R, M), dtype=np.int32), wsum=np.empty(R))
+    if counts:
+        o['counts'] = np.empty((R, N), dtype=np.int32)
+    if x is not None:
+        o['x'] = np.empty((R, M, x.shape[1]))
+    return o
+
+
+def _equal_x(x, N):
+    """The rows to gather as the C API takes them (N x k float64), or None."""
+    if x is None:
+        return None
+    x = f64(x)
+    if x.ndim != 2 or len(x) != N or x.shape[1] < 1:
+        raise ValueError("the rows to gather must be an array of shape (%d, k)" % N)
+    return x
+
+
+def _equal_done(o):
+    o['idx'] = o['idx'].astype(np.int64)
+    if 'counts' in o:
+        o['counts'] = o['counts'].astype(np.int64)
+    return o
+
+
+def resample_equal(w, M, seed, chain0=0, x=None, counts=False, ctx=None):
+    """M equal-weight draws from each of R weight vectors w (R x N; finite, >= 0, positive sum) by the reference's
+    systematic resampling, with its rounding (resample_equal, utils.py:1120-1187); vector r uses the B2N stream (seed,
+    chain0 + r).  Returns dict(idx (R x M, int64): the drawn samples in random order, wsum (R): the sequential sum of
+    each vector) and, with counts=True, counts (R x N, int64): the times each sample is drawn; with x (N x k), x (R x M
+    x k): its rows x[idx]."""
+    ctx = _ctx(ctx)
+    w = f64(np.atleast_2d(w))
+    R, N = w.shape
+    x = _equal_x(x, N)
+    o = _equal_outputs(R, N, int(M), x, counts)
+    ctx.check(ctx.lib.b2n_resample_equal(ctx.h, ptr(w), N, R, int(M), int(seed), int(chain0), ptr(x),
+                                         0 if x is None else x.shape[1], ptr(o['idx']), ptr(o.get('counts')),
+                                         ptr(o['wsum']), ptr(o.get('x'))))
+    return _equal_done(o)
+
+
+def jitter_equal(logl, samples_n, R, M, seed, chain0=0, approx=False, logwt_ref=None, logz_ref=None, x=None,
+                 counts=False, logrwt=None, ctx=None):
+    """jitter_runs plus, per realisation, M equal-weight draws over the record's samples under its weights
+    exp(logwt - logz[-1]) (resample_equal's outputs above).  The draws of realisation r use the stream (seed,
+    EQUAL_CHAIN0 + chain0 + r).  logwt_ref / logz_ref (the record's own) are required.  logrwt: as in jitter_runs."""
+    ctx = _ctx(ctx)
+    logl, n_, wref = _jitter_record(logl, samples_n, logwt_ref, True)
+    N, R = len(logl), int(R)
+    x = _equal_x(x, N)
+    rw = None if logrwt is None else _logrwt(logrwt, N)
+    o = _summaries(R, True)
+    o.update(_equal_outputs(R, N, int(M), x, counts))
+    _set_reweight(ctx, rw)
+    ctx.check(ctx.lib.b2n_jitter_equal(ctx.h, ptr(logl), ptr(n_), N, ptr(wref), float(logz_ref), int(bool(approx)), R,
+                                       int(seed), int(chain0), int(M), ptr(x), 0 if x is None else x.shape[1],
+                                       ptr(o['logz']), ptr(o['logzerr']), ptr(o['h']), ptr(o['kld']), ptr(o['idx']),
+                                       ptr(o.get('counts')), ptr(o['wsum']), ptr(o.get('x'))))
+    return _equal_done(o)
+
+
+def resample_equal_runs(logl, strand, base, piece_ptr, piece_strand, end, R, M, seed, chain0=0, logwt_ref=None,
+                        logz_ref=None, x=None, counts=False, logrwt=None, ctx=None):
+    """resample_runs plus, per realisation, M equal-weight draws over the record's samples, each weighted by the sum
+    of its copies' exp(logwt - logz[-1]) (a sample drawn 0 times is never drawn).  The draws of realisation r use the
+    stream (seed, EQUAL_CHAIN0 + chain0 + r).  logwt_ref / logz_ref (the record's own) are required.  logrwt: as in
+    resample_runs."""
+    ctx = _ctx(ctx)
+    logl = f64(logl)
+    N = len(logl)
+    strand, base, pp, ps, end = _strand_record(N, strand, base, piece_ptr, piece_strand, end)
+    S, R = len(base), int(R)
+    wref = _logwt_ref(logwt_ref, N)
+    x = _equal_x(x, N)
+    rw = None if logrwt is None else _logrwt(logrwt, N)
+    o = _summaries(R, True)
+    o.update(_equal_outputs(R, N, int(M), x, counts))
+    _set_reweight(ctx, rw)
+    ctx.check(ctx.lib.b2n_resample_equal_runs(ctx.h, ptr(logl), ptr(strand), N, S, ptr(base), ptr(pp), ptr(ps),
+                                              ptr(end), ptr(wref), float(logz_ref), R, int(seed), int(chain0), int(M),
+                                              ptr(x), 0 if x is None else x.shape[1], ptr(o['logz']),
+                                              ptr(o['logzerr']), ptr(o['h']), ptr(o['kld']), ptr(o['idx']),
+                                              ptr(o.get('counts')), ptr(o['wsum']), ptr(o.get('x'))))
+    return _equal_done(o)
+
+
 def merge_runs(logl, samples_n, run_ptr, nbase, lowedge=None, arrays=True, ctx=None):
     """R records merged into one (merge_runs / _merge_two, utils.py:1817-1900, 2045-2225; include/b200nest.h,
     b2n_merge_runs).  logl / samples_n: the records concatenated, run r = [run_ptr[r], run_ptr[r + 1]), each run's

@@ -8,11 +8,13 @@ What is mirrored (reference py/dynesty/utils.py, same names / meaning):
   merge_runs    :1817-1929   several runs merged into one (``b2n_merge_runs``)
   mean_and_cov  :1081-1117   weighted mean and covariance (``b2n_weighted_stats``)
   quantile      :1196-1233   weighted quantiles (``b2n_weighted_stats``; unweighted: np.percentile)
+  resample_equal :1120-1187  equal-weight draws by systematic resampling (``b2n_resample_equal``)
   reweight_run  :1663-1708   a run's weights for a new target (``b2n_compute_integrals``)
 and the batched forms the dynamic sampler's stopping function needs: ``jitter_realisations`` (``b2n_jitter_runs``) and
 ``resample_realisations`` (``b2n_resample_runs``), n_mc realisations in one call and a fixed number of kernel launches,
 and ``posterior_realisations``: the same realisations with the posterior mean, covariance and quantiles of each
-(``b2n_jitter_posterior`` / ``b2n_resample_posterior``).
+(``b2n_jitter_posterior`` / ``b2n_resample_posterior``), and ``equal_realisations``: equal-weight draws of each
+(``b2n_jitter_equal`` / ``b2n_resample_equal_runs``).
 
 Randomness: realisation r of a call is the B2N Philox stream (seed, chain0 + r) (include/b200nest.h), so a (seed,
 chain) pair names one realisation: it is the same whether it is computed alone or in a batch of any size.
@@ -30,6 +32,7 @@ reference's rule; for the device rounds, which remove `batch` points at once, it
 where the reference's rule would count every slot as occupied.
 """
 import math
+import warnings
 
 import numpy as np
 
@@ -336,6 +339,77 @@ def posterior_realisations(res, n_mc, seed, chain0=0, error='jitter', approx=Fal
                                     ctx=ctx, **_rw(res))
     return ops.resample_posterior(*_strand_inputs(res)[1], x, int(n_mc), int(seed), chain0=int(chain0),
                                   logwt_ref=res['logwt'], logz_ref=logz_ref, q=q, ctx=ctx, **_rw(res))
+
+
+# ---------------------------------------------------------------------------------------------- equal-weight samples
+SQRTEPS = math.sqrt(float(np.finfo(np.float64).eps))
+EQUAL_MAX_BYTES = 8 << 30       # the largest gathered output equal_realisations returns (n_mc x nsamples x k float64)
+
+
+def resample_equal(samples, weights, rstate=None, seed=None, chain=0, ctx=None):
+    """resample_equal (utils.py:1120-1187): len(weights) equal-weight draws of samples, in random order, by systematic
+    resampling -- each sample appears floor(N w_i) or ceil(N w_i) times -- computed on the GPU with the reference's
+    rounding (b2n_resample_equal).  The draw is the B2N stream (seed, chain); with a numpy Generator rstate and no seed
+    the seed is rstate.integers(2**63), with neither a fresh one.  Warns, as the reference does, when the weights do not
+    sum to 1 within sqrt(eps); they are then renormalised.  Where the reference raises IndexError (a position that
+    rounds to 1.0) the last sample is drawn."""
+    w = np.asarray(weights, dtype=np.float64)
+    if w.ndim != 1 or len(w) < 1:
+        raise ValueError("weights must be a non-empty 1-d array")
+    if len(samples) != len(w):
+        raise ValueError("Dimension mismatch: len(weights) != len(samples).")
+    if not np.isfinite(w).all() or (w < 0).any():
+        raise ValueError("weights must be finite and non-negative")
+    if not (w > 0).any():
+        raise ValueError("weights sum to zero")
+    if seed is None:
+        seed = int(rstate.integers(1 << 63)) if rstate is not None else _seed(None)
+    o = ops.resample_equal(w[None, :], len(w), int(seed), chain0=int(chain), ctx=ctx)
+    if abs(o['wsum'][0] - 1.) > SQRTEPS:
+        warnings.warn("Weights do not sum to 1 and have been renormalized.")
+    return np.asarray(samples)[o['idx'][0]]
+
+
+def equal_realisations(res, n_mc, seed, chain0=0, error='jitter', nsamples=None, approx=False, of=None, ctx=None):
+    """n_mc realisations of `res` -- jitter_run's (error='jitter') or resample_run's (error='resample') -- each turned
+    into nsamples (default: the record's length) equal-weight draws of the record's samples by resample_equal's
+    algorithm.  Returns the dict of jitter_realisations / resample_realisations (logz, logzerr, h, kld; n_mc values
+    each) plus idx (n_mc x nsamples): the drawn rows of the record, in random order, and wsum (n_mc): the sum of each
+    realisation's weights exp(logwt - logz[-1]) (on the resample path, a row's weight is the sum over its copies).
+    With of='samples' or 'blob', also that key: res[of][idx] (n_mc x nsamples x k), gathered on the GPU; it may not
+    exceed EQUAL_MAX_BYTES.  Realisation r is the one jitter_run(res, seed, chain0 + r) / resample_run(res, seed,
+    chain0 + r) returns; its draws use the stream (seed, ops.EQUAL_CHAIN0 + chain0 + r), so row r is the same whatever
+    n_mc.  resample_run(res).samples_equal() would draw over the copies as rows of their own: the same distribution,
+    not the same bits."""
+    if error not in ('jitter', 'resample'):
+        raise ValueError("Input `'error'` option '{}' is not valid.".format(error))
+    if of not in (None, 'samples', 'blob'):
+        raise ValueError("of must be None, 'samples' or 'blob', not %r" % (of,))
+    logl = np.asarray(res['logl'], dtype=float)
+    N, R = len(logl), int(n_mc)
+    M = N if nsamples is None else int(nsamples)
+    if M < 1 or R < 1:
+        raise ValueError("n_mc and nsamples must be positive")
+    if R * M >= 1 << 31:
+        raise ValueError("n_mc x nsamples must be below 2^31")
+    x = None
+    if of is not None:
+        x = np.asarray(res[of]) if of in res else np.empty((0, 0))
+        if x.ndim != 2 or len(x) != N or x.shape[1] < 1:
+            raise ValueError("equal_realisations(of=%r) needs res[%r] with one row per sample" % (of, of))
+        if R * M * x.shape[1] * 8 > EQUAL_MAX_BYTES:
+            raise ValueError("the gathered rows (n_mc x nsamples x %d float64) would exceed %d bytes; gather "
+                             "res[%r][idx] in pieces instead" % (x.shape[1], EQUAL_MAX_BYTES, of))
+    logz_ref = _logz_end(res)
+    if error == 'jitter':
+        o = ops.jitter_equal(logl, samples_n_of(res), R, M, int(seed), chain0=int(chain0), approx=approx,
+                             logwt_ref=res['logwt'], logz_ref=logz_ref, x=x, ctx=ctx, **_rw(res))
+    else:
+        o = ops.resample_equal_runs(*_strand_inputs(res)[1], R, M, int(seed), chain0=int(chain0),
+                                    logwt_ref=res['logwt'], logz_ref=logz_ref, x=x, ctx=ctx, **_rw(res))
+    if of is not None:
+        o[of] = o.pop('x')
+    return o
 
 
 # ---------------------------------------------------------------------------------------------- merging runs

@@ -444,6 +444,52 @@ int b2n_resample_posterior(b2n_ctx* ctx, const double* logl, const int32_t* stra
                            uint64_t chain0, const double* x, int32_t n, const double* q, int32_t nq, double* logz,
                            double* logzerr, double* h, double* kld, double* mean, double* cov, double* quant);
 
+/* ---- equal-weight posterior samples (utils.py:895-903 samples_equal, :1120-1187 resample_equal) ------------------
+ * R weight vectors over one set of N samples, each turned into M equal-weight draws by the reference's systematic
+ * resampling, with its rounding (DESIGN.md section 15.5).  For vector r, on the B2N stream (seed, chain):
+ *   tick 0   one uniform u (rstate.random());
+ *   c        the SEQUENTIAL left-to-right FP64 cumsum of w (np.cumsum's order), wsum = c[N-1], C_j = c_j / wsum;
+ *   pos_i    = (u + i) / M, that add then that divide, i = 0..M-1;
+ *   draw_i   = the smallest j with pos_i < C_j.  A position that rounds to 1.0 (possible only when u + M - 1 rounds
+ *              up to M) takes N - 1, where the reference raises IndexError;
+ *   tick 1   one uniform vector event of M elements; perm = its stable argsort (rstate.permutation: ties, of
+ *            probability ~2^-53, by index; no event is drawn for M == 1 in the oracle, and none is needed);
+ *   idx[t]   = draw[perm[t]].
+ * counts[j] = the times sample j is drawn: floor(M w_j / wsum) or its ceiling.  A sample of weight 0 is never drawn
+ * (a weight of -0.0 counts as 0).  idx points at rows of the record; xout[t] = x[idx[t]] (k values a row).
+ * The cumsum runs one thread per vector over N (the N x R weights are read coalesced across vectors); counts come
+ * from an estimate of each boundary's first position, corrected with the same pos_i; each position finds its sample by
+ * bisection.  No float atomics; vector r's outputs do not depend on R.  A fixed number of kernel launches (3, 4 with
+ * counts, plus those of one CUB segmented radix sort) whatever N, M or R.
+ * Refused with B2N_ERR_ARG: N or M < 1 or >= 2^31, R < 1 or > 65535, R * M >= 2^31, x NULL with k > 0 or xout
+ * given, k < 0; and, after the device has checked the weights (these calls therefore synchronise), a weight that
+ * is negative, NaN or inf, or a vector whose sum is 0 or inf.
+ * Outputs: idx (R x M int32), counts (R x N int32, may be NULL), wsum (R, may be NULL), xout (R x M x k, may be
+ * NULL), row-major.
+ *
+ * b2n_resample_equal: the weights given, w (R x N, row-major); vector r uses the stream (seed, chain0 + r).  w and x
+ * host or device like the outputs. */
+int b2n_resample_equal(b2n_ctx* ctx, const double* w, int64_t N, int32_t R, int64_t M, uint64_t seed, uint64_t chain0,
+                       const double* x, int32_t k, int32_t* idx, int32_t* counts, double* wsum, double* xout);
+/* b2n_jitter_equal / b2n_resample_equal_runs: the realisations of b2n_jitter_runs / b2n_resample_runs (same record
+ * arguments and streams, summaries logz, logzerr, h, kld bit for bit, and a pending b2n_set_reweight read the same
+ * way), each turned into M equal-weight draws over the record's rows as above.  The weights are those of
+ * b2n_jitter_posterior / b2n_resample_posterior: w_ri = exp(logwt_ri - logz_r[-1]); on the resample path the sum over
+ * sample i's copies (a sample drawn 0 times has weight -0.0).  So the resample path draws record rows, where the
+ * reference's resample_run(res).samples_equal() draws over the copies as rows of their own: the same distribution,
+ * not the same bits.  Realisation r's draw uses the stream (seed, B2N_EQUAL_CHAIN0 + chain0 + r), disjoint from the
+ * realisation's own (seed, chain0 + r).  logwt_ref is required (kld). */
+#define B2N_EQUAL_CHAIN0 (1ull << 62)
+int b2n_jitter_equal(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, int64_t N, const double* logwt_ref,
+                     double logz_ref, int32_t approx, int32_t R, uint64_t seed, uint64_t chain0, int64_t M,
+                     const double* x, int32_t k, double* logz, double* logzerr, double* h, double* kld, int32_t* idx,
+                     int32_t* counts, double* wsum, double* xout);
+int b2n_resample_equal_runs(b2n_ctx* ctx, const double* logl, const int32_t* strand, int64_t N, int32_t S,
+                            const uint8_t* base, const int64_t* piece_ptr, const int32_t* piece_strand,
+                            const uint8_t* end, const double* logwt_ref, double logz_ref, int32_t R, uint64_t seed,
+                            uint64_t chain0, int64_t M, const double* x, int32_t k, double* logz, double* logzerr,
+                            double* h, double* kld, int32_t* idx, int32_t* counts, double* wsum, double* xout);
+
 /* ---- merge_runs (utils.py:1817-1900, _merge_two :2045-2225 of the reference) ---------------------------------------
  * R dead-point records of N samples in all, concatenated: run r is samples [run_ptr[r], run_ptr[r + 1]), its logl
  * ascending and free of NaN (assumed, not checked), samples_n its live count at every sample (>= 1).  The first nbase
@@ -487,9 +533,11 @@ int b2n_merge_runs(b2n_ctx* ctx, const double* logl, const int64_t* samples_n, c
 int b2n_compute_integrals(b2n_ctx* ctx, const double* logl, const double* logvol, const double* logrwt, int64_t N,
                           double* last3, double* logwt, double* logz, double* logzvar, double* h);
 /* b2n_set_reweight: the log-reweight (N, host or device like the arrays of the call) for the NEXT b2n_jitter_runs /
- * b2n_resample_runs / b2n_jitter_posterior / b2n_resample_posterior call, whose realisations then carry it as above
+ * b2n_resample_runs / b2n_jitter_posterior / b2n_resample_posterior / b2n_jitter_equal / b2n_resample_equal_runs
+ * call, whose realisations then carry it as above
  * (one call, then reset, however that call ends; the array must stay valid until then).  That call needs the same N,
- * else it fails with B2N_ERR_ARG.  b2n_merge_runs, b2n_weighted_stats and b2n_compute_integrals called with a
+ * else it fails with B2N_ERR_ARG.  b2n_merge_runs, b2n_weighted_stats, b2n_resample_equal and b2n_compute_integrals
+ * called with a
  * reweight pending clear it and return B2N_ERR_UNSUPPORTED.  NULL cancels.  The realisation entry points keep their
  * launch counts; with the reweight they run the _rw instantiations of the same passes. */
 int b2n_set_reweight(b2n_ctx* ctx, const double* logrwt, int64_t N);
